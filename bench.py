@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — CUP2D hot path on B200: Mcell-updates/s (advect+diffuse+Poisson iter) at 8192^2.
+"""bench.py — CUP2D hot path on H100: Mcell-updates/s (advect+diffuse+Poisson iter) at 8192^2.
 
 One "step" = one full time step of the hot path on a uniform grid without bodies:
     dt control (umax reduction) -> RK2 (two fused WENO5 advect-diffuse stages) -> Poisson RHS ->
@@ -7,7 +7,7 @@ One "step" = one full time step of the hot path on a uniform grid without bodies
     hard-coded cap, main.cpp:7028-7030 / cuda.cu:438) -> pressure correction.
 cell-updates per step = cells * (2 stage sweeps + K Poisson iterations)   [the metric's own definition]
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--level L] [--poisson-iters K] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--level L] [--poisson-iters K] [--impl reference] [--dump-outputs DIR]
 
 N > 1: launched by torchrun, one rank per GPU; the 8192^2 grid is split into contiguous Hilbert ranges
 (strong scaling); halos and Krylov dots go over NVLink peer memory inside the library's kernels.
@@ -45,25 +45,19 @@ ALG_BYTES = {
 }
 
 
-def load_traffic():
-    """measured DRAM bytes per cell per launch of each kernel (ncu --set full, profiles/traffic.json)"""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
-
-
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 class ClockSampler:
     """nvidia-smi clocks/throttle reasons sampled while the timed region runs."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -93,7 +87,7 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             f = [x.strip() for x in r.split(",")]
@@ -107,8 +101,12 @@ class ClockSampler:
             for n, v in zip(names, f[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(n)
+            try:
+                plim.append(float(f[7]))
+            except (IndexError, ValueError):
+                pass
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "samples": len(sm), "reasons": sorted(reasons)}
+                "power_limit_w": max(plim) if plim else None, "samples": len(sm), "reasons": sorted(reasons)}
 
 
 def gpu_visible():
@@ -149,7 +147,7 @@ def cpu_composite(level, reps, kiter):
     """The reference's own path on a bounded sample.  Operators = unmodified main.cpp under OpenMP on the host threads this
     process may use.  The reference has no CPU Poisson solver (cuda.cu is its only one), so `value` always uses the CPU
     restatement of cuda.cu for the Poisson iterations (one fixed definition: the figure never switches solver), and the
-    composite with the reference's own GPU solver on this box's B200 is reported beside it as `with_reference_gpu_solver`."""
+    composite with the reference's own GPU solver on this box's GPU is reported beside it as `with_reference_gpu_solver`."""
     threads = usable_cpus()
     reps = max(5, reps)
     run_harness_time(HARNESS, 3, 1, 1, threads, timeout=120)           # warm: binary and OpenMP runtime paged in
@@ -169,7 +167,7 @@ def cpu_composite(level, reps, kiter):
         "poisson_solver": "cpu_restatement",
         "operator_seconds_min_med_max": t.get("min_med_max"),
     }
-    # named extra: the same composite with the reference's own cuda.cu (cuSPARSE/cuBLAS) iterating on the B200
+    # named extra: the same composite with the reference's own cuda.cu (cuSPARSE/cuBLAS) iterating on the GPU
     extra = {"unavailable": "no GPU visible or reference GPU binary not built"}
     if os.path.exists(HARNESS_GPU) and gpu_visible():
         try:
@@ -180,7 +178,7 @@ def cpu_composite(level, reps, kiter):
                      "poisson_iter_Mcells_s": tg["cells"] / tg["t_poisson_iter"] / 1e6,
                      "value_min_median_max": {"min": _composite(tg, kiter, 2)[0], "median": _composite(tg, kiter, 1)[0],
                                               "max": _composite(tg, kiter, 0)[0]},
-                     "poisson_solver": "reference cuda.cu on 1 B200 (host<->device copies of x,b per solve included, as the reference does)"}
+                     "poisson_solver": "reference cuda.cu on 1 GPU (host<->device copies of x,b per solve included, as the reference does)"}
         except Exception as e:
             extra = {"unavailable": f"{type(e).__name__}: {e}"[:200]}
     out["with_reference_gpu_solver"] = extra
@@ -238,8 +236,28 @@ def multi_gpu_parity(cup2d_b200, np, torch, dist, rank, world, local_rank, K):
     return out[0]
 
 
-# FP64 instructions the advect stage executes per cell (DFMA + DMUL + DADD of the ncu instruction mix; round 1: 189)
+# FP64 instructions the advect stage executes per cell (DFMA + DMUL + DADD of the ncu instruction mix)
 ADVECT_FP64_PER_CELL = 152.4
+
+DUMP_SAMPLE_CELLS = 1 << 20   # cells per rank sampled by --dump-outputs: 3 fields + index in float64 = 32 MB
+
+
+def dump_outputs(out_dir, sim, np, rank, world, result):
+    """What the timed path hands its caller after its last step, as float64 .npy files: the step result (dt, Poisson
+    iterations, residual) and u, v, p at a fixed, seeded sample of this rank's cells (cell_index = 64*block + 8*iy + ix in
+    the library's block order).  The sample depends only on the grid and the rank count, so two builds compare cell for cell."""
+    os.makedirs(out_dir, exist_ok=True)
+    ncell = int(sim.nloc) * 64
+    m = min(ncell, DUMP_SAMPLE_CELLS // world)
+    idx = np.arange(ncell) if m == ncell else np.sort(np.random.default_rng(0).choice(ncell, m, replace=False))
+    vel = sim.download_blocks("vel").reshape(ncell, 2)
+    pres = sim.download_blocks("pres")
+    arrays = {"step_result": np.array(result, dtype=np.float64), "cell_index": idx, "u": vel[idx, 0], "v": vel[idx, 1],
+              "p": pres[idx]}
+    sfx = f"_rank{rank}" if world > 1 else ""
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + sfx + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+    return sorted(arrays)
 
 
 def main():
@@ -256,6 +274,8 @@ def main():
     ap.add_argument("--no-pipeline", action="store_true", help="skip the pipelined end-to-end figure")
     ap.add_argument("--no-graph", action="store_true", help="launch every kernel from the host instead of replaying the step graph")
     ap.add_argument("--profile-steps", type=int, default=5, help="steps of the separate, event-instrumented pass (per-kernel table)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the last step's result and a seeded "
+                                                          "sample of its velocity and pressure to DIR/<name>.npy (float64)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -272,7 +292,7 @@ def main():
                       f"iterations (tol 0) + pressure correction; one CUDA-graph launch per step, no host synchronisation inside the timed region",
               "cell_updates_per_step": f"cells*(2+{K})", "poisson_iters": K,
               "partition": f"{world} contiguous Hilbert range(s), halo + dots over NVLink peer memory" if world > 1 else "single GPU",
-              "cache": "inputs larger than L2 (each field >= 0.5 GB vs 126 MB L2)" if L >= 9 else "L2-resident at this size"}
+              "cache": "inputs larger than L2 (each field >= 0.13 GB vs 50 MB L2)" if L >= 8 else "L2-resident at this size"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -305,6 +325,7 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("bench.py: no CUDA device; cup2d_b200 has no CPU fallback")
     torch.cuda.set_device(local_rank)
+    n_sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
     dist = None
     parity = None
     if world > 1:
@@ -390,6 +411,7 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     launches = sim.launch_count() - l0
     dt_last, it_last, err_last = sim.step_result()
+    dumped = dump_outputs(args.dump_outputs, sim, np, rank, world, (dt_last, it_last, err_last)) if args.dump_outputs else None
     ms_per_step = ms / args.steps
     value = cells * (2 + K) / (ms_per_step * 1e-3) / 1e6
 
@@ -491,10 +513,8 @@ def main():
     top = kernels[0] if kernels else None
     roofline = None
     if top:
-        tr = load_traffic().get(top["kernel"])
         roofline = {"kernel": top["kernel"], "bound": "hbm", "achieved": top["achieved_GBs"], "peak": peak,
                     "unit": "GB/s", "frac": top["frac_hbm"],
-                    "traffic": tr * cells_loc if tr else None, "traffic_unit": "bytes per launch (ncu dram read+write, profiles/)",
                     "peak_source": peak_src,
                     "ms_per_launch": top["ms_per_launch"], "share_of_step": top["share_of_step"],
                     "timed": "CUDA events around every launch in a separate instrumented pass of the same steps (kernel-by-kernel launches)"}
@@ -505,12 +525,12 @@ def main():
     if adv:
         # the north-star kernel: HBM fraction and the FP64-pipe bound it actually sits under
         gcell = cells_loc / (adv["ms_per_launch"] * 1e-3) / 1e9
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1920.0
-        fp64_floor_ms = cells_loc * ADVECT_FP64_PER_CELL / 32.0 / (148 * 2 * sm_mhz * 1e6) * 1e3   # 2 FP64 warp-instr/clk/SM
+        sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
+        fp64_floor_ms = cells_loc * ADVECT_FP64_PER_CELL / 32.0 / (n_sms * 2 * sm_mhz * 1e6) * 1e3   # 2 FP64 warp-instr/clk/SM
         extra["advect_stage"] = {"Gcell_per_s": gcell, "achieved_GBs": adv["achieved_GBs"], "frac_hbm": adv["frac_hbm"],
                                  "ms_per_launch": adv["ms_per_launch"], "alg_bytes_per_cell": 48.0,
                                  "fp64_floor_ms": fp64_floor_ms, "frac_fp64_floor": fp64_floor_ms / adv["ms_per_launch"],
-                                 "note": f"bound by the FP64 pipe, not HBM: {ADVECT_FP64_PER_CELL:g} FP64 instr/cell (ncu, profiles/r02g_advect_ncu.md) at 64 lanes/clk/SM; see DESIGN.md 3.1"}
+                                 "note": f"FP64-pipe floor: {ADVECT_FP64_PER_CELL:g} FP64 instr/cell at 64 lanes/clk/SM on {n_sms} SMs; see DESIGN.md 3.1"}
         # SURVEY 8(d)(ii): one full RK2 step = the two fused stages (vold = vel is a pointer swap, not a copy)
         try:
             rk2_ms = adv["ms_per_launch"] * adv["launches_per_step"]
@@ -546,7 +566,9 @@ def main():
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": config, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
             "roofline": roofline, "kernels": kernels, "cpu_baseline": cpu, "dt": dt_last, "poisson_residual": err_last,
-            "graph": not args.no_graph}
+            "graph": not args.no_graph, "gpu": torch.cuda.get_device_name(local_rank)}
+    if dumped:
+        line["dumped_outputs"] = {"dir": args.dump_outputs, "arrays": dumped}
     if parity is not None:
         line["parity"] = parity
     line.update(extra)

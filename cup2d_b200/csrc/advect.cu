@@ -31,7 +31,7 @@ namespace cup2d {
 #ifndef CUP2D_ADV_LDGSTS
 // 1: the tile is filled by 16-byte cp.async (SASS LDGSTS) issued by all threads, 13 per thread;  0: by per-row bulk copies
 // (SASS UBLKCP + mbarrier).  A bulk copy issued by a divergent thread costs ~8 warp instructions (ELECT/R2UR loop over the
-// lanes) and a tile needs 216 of them: 0.914 ms per stage against 0.846 ms with cp.async at 8192^2 (profiles/r02e_variants.jsonl).
+// lanes) and a tile needs 216 of them, which makes the bulk-copy fill the slower one.
 #define CUP2D_ADV_LDGSTS 1
 #endif
 

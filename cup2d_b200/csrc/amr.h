@@ -25,6 +25,8 @@ int cup2d_amr_laplacian_fast(cup2d_amr *a, double dt);
 
 namespace cup2d {
 
+constexpr int AMR_GRID_SMS = 132; // SMs of an H100 SXM: the grid-stride launches of this path are capped at a few waves of them
+
 struct Csr {
   int64_t *rowptr = nullptr;
   int *src_block = nullptr, *src_cc = nullptr;

@@ -1,7 +1,7 @@
 // Advect-diffuse right-hand side on multi-level meshes, per-block lab loader on the WENO line core (DESIGN.md 7.1 step 1).
 //
-// STATUS: like csrc/amr_ops.cu — compiled for sm_100a, its logic checked on the CPU through tests/host_emu/ (cooperative
-// thread emulation), NOT YET RUN ON HARDWARE.  cup2d_amr_advect_diffuse_rhs_fast gives the same result as the table-gather
+// STATUS: like csrc/amr_ops.cu — compiled for sm_90a, its logic also checked on the CPU through tests/host_emu/ (cooperative
+// thread emulation).  cup2d_amr_advect_diffuse_rhs_fast gives the same result as the table-gather
 // baseline cup2d_amr_advect_diffuse_rhs.
 //
 // One warp owns four blocks.  Per block two padded planes (u, v: 14 rows x 15) in shared memory hold the lab:

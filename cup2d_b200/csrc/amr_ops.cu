@@ -1,7 +1,7 @@
 // Stencil operators on multi-level (block-AMR) meshes — FIRST, CORRECTNESS-ORIENTED DEVICE PATH (SURVEY §8(f) rank 2).
 //
-// STATUS: validated on hardware in round 2 (tests/test_gpu_amr.py green on a B200, compute-sanitizer memcheck / racecheck
-// clean: profiles/r02a_first_contact.md).  See DESIGN.md 7.1 for the plan this is step 0 of.
+// STATUS: checked on the GPU by tests/test_gpu_amr.py and on the CPU by the host emulation (tests/host_emu/).  See DESIGN.md
+// 7.1 for the plan this is step 0 of.
 //
 // Shape (deliberately the simplest thing that can be compared with the reference, not the fast design):
 //   1. lab = T . field : the ghost-stencil tables of the host plan (csrc/amr_plan.cpp) applied as a CSR gather into a
@@ -254,7 +254,7 @@ __global__ void amr_fluxcorr_kernel(const CoarseFace *__restrict__ cf, int ncf, 
   *dst = v;
 }
 
-static int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, 148 * 16); }
+static int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, AMR_GRID_SMS * 16); }
 
 static int upload_csr(cup2d_amr *a, int which) {
   int64_t nnz = cup2d_amr_plan_stencil(a->plan, which, nullptr, nullptr, nullptr, nullptr);

@@ -9,8 +9,8 @@
 //   cup2d_amr_udef_assemble   : tmpV = sum of u_def where the shape's chi is not below the field's (6980-7002): bit-identical
 // Also here, because it needs the same per-block (i, j, h) tables: cup2d_amr_dump, dump()'s three files from a multi-level mesh
 // (main.cpp:3367-3467), byte for byte.
-// STATUS: like the rest of the multi-level device path, written after the round's GPU budget was spent — compiled for
-// sm_100a, run under the host emulation only.
+// STATUS: like the rest of the multi-level device path: compiled for sm_90a, its logic also checked on the CPU through
+// the host emulation (tests/host_emu/).
 #include "sim.h"
 #include "amr.h"
 #include <algorithm>
@@ -134,7 +134,7 @@ amr_dump_pack_kernel(const double *__restrict__ vel, const int2 *__restrict__ ij
 }
 
 static AmrShapeView view_of(const cup2d_amr::Shape &sh) { return AmrShapeView{sh.d_ids, sh.d_X, sh.d_udef, sh.nob}; }
-static int ob_grid(int nob) { return std::max(1, std::min((nob + 3) / 4, 148 * 8)); }
+static int ob_grid(int nob) { return std::max(1, std::min((nob + 3) / 4, AMR_GRID_SMS * 8)); }
 
 static int ensure_ij(cup2d_amr *a) {
   if (a->d_ij) return CUP2D_OK;
@@ -264,7 +264,7 @@ int cup2d_amr_dump(cup2d_amr *a, double time, const char *path) {
   for (int64_t b0 = 0; rc == CUP2D_OK && b0 < a->nb; b0 += CHUNK) {
     const int nb = (int)std::min<int64_t>(CHUNK, a->nb - b0);
     const size_t ncell = (size_t)nb * 64;
-    amr_dump_pack_kernel<<<(int)std::min<size_t>((ncell + 255) / 256, 148 * 8), 256, 0, a->stream>>>(
+    amr_dump_pack_kernel<<<(int)std::min<size_t>((ncell + 255) / 256, AMR_GRID_SMS * 8), 256, 0, a->stream>>>(
         a->f[CUP2D_VEL], reinterpret_cast<const int2 *>(a->d_ij), a->d_h, (int)b0, nb, reinterpret_cast<float4 *>(d_buf), d_buf + nx);
     cudaMemcpyAsync(h_buf, d_buf, ncell * 8 * sizeof(float), cudaMemcpyDeviceToHost, a->stream);
     cudaMemcpyAsync(h_buf + nx, d_buf + nx, ncell * 3 * sizeof(float), cudaMemcpyDeviceToHost, a->stream);

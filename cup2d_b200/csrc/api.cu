@@ -290,8 +290,8 @@ int cup2d_create(const cup2d_config *cfg, cup2d_sim **out) {
   CUP2D_CUDA(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CUP2D_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) {
-    set_error(std::string("cup2d_create: device '") + prop.name + "' is not sm_100 (compiled for sm_100a only)");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error(std::string("cup2d_create: device '") + prop.name + "' is not sm_90 (compiled for sm_90a only)");
     return CUP2D_ENOGPU;
   }
   cup2d_sim *s = nullptr;
@@ -323,8 +323,8 @@ int cup2d_poisson_create(int64_t nblocks, const int32_t *nbr, int32_t device, cu
   CUP2D_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUP2D_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error(std::string("cup2d_poisson_create: device '") + prop.name + "' is not sm_100");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error(std::string("cup2d_poisson_create: device '") + prop.name + "' is not sm_90");
     return CUP2D_ENOGPU;
   }
   cup2d_sim *s = new cup2d_sim;
@@ -456,8 +456,8 @@ int cup2d::poisson_create_general_ranks_ex(int64_t nblocks_global, int32_t rank,
   CUP2D_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUP2D_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error(std::string("cup2d_poisson_create_general_ranks: device '") + prop.name + "' is not sm_100");
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error(std::string("cup2d_poisson_create_general_ranks: device '") + prop.name + "' is not sm_90");
     return CUP2D_ENOGPU;
   }
   cup2d_sim *s = new cup2d_sim;

@@ -1,4 +1,4 @@
-// Internal helpers shared by the kernels of libcup2d_b200.so (sm_100a only).
+// Internal helpers shared by the kernels of libcup2d_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

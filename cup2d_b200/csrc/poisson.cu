@@ -337,16 +337,15 @@ k_spmv(const double *__restrict__ z, const double *__restrict__ d, double *__res
   double *sw = s_scr + warp * SCRW;
   for (int row0 = (blockIdx.x * WPB + warp) * 32; row0 < nrows; row0 += gridDim.x * WPB * 32) {
     const int nv = min(32, nrows - row0);
-    // uniform grids: both global loads are issued before any shared-memory work (memory-level parallelism,
-    // -4 % per iteration in profiles/r01h); with general rows the extra live registers cost more than that
+    // uniform grids: both global loads are issued before any shared-memory work (memory-level parallelism); with general
+    // rows the extra live registers cost more than that
     constexpr bool HOIST = !IRR;
     double2 cz[4], ca[4], cd[4];
     chunk_ld(z, row0, nv, lane, cz);
     if (HOIST) chunk_ld(d, row0, nv, lane, cd);
     double zz[8], az[8];
-    // one GPU: the cooperative form (rows.cuh; measured r02k/r02l).  Several ranks keep the plain form, which is the code
-    // that ran on 2, 4 and 8 GPUs (r02i/r02j); the cooperative form handles halo slots too (emulated 2-rank tests) but has
-    // not been timed or run on more than one GPU
+    // one GPU: the cooperative form (rows.cuh).  Several ranks keep the plain form; the cooperative form handles halo
+    // slots too (emulated 2-rank tests) but has not been timed or run on more than one GPU
     if (COOP) rows_lap_coop(cz, z, row0, nv, nbr, sw, lane, zz, az, IRR ? irr : IrrView(), gate);
     else rows_lap_c(cz, z, row0, nv, nbr, sw, lane, zz, az, IRR ? irr : IrrView(), gate);
     // back to chunk layout: the dots and the store are element-wise

@@ -3,8 +3,7 @@
 // Compute mapping ("row layout"): one lane owns one row of 8 cells of one 8x8 block (8 lanes = one
 // block, one warp = 4 consecutive blocks = 32 rows = one CHUNK of 2 KB (scalar) / 4 KB (vector) of
 // CONTIGUOUS memory).  If every lane read its own row with 128-bit loads, each load instruction would
-// touch 16-32 different 128-B lines and the kernels become L1/TEX-bound (measured: 78-98 % l1tex
-// throughput, profiles/r01_summary.md).  So global memory is only ever touched in "chunk layout": lane
+// touch 16-32 different 128-B lines and the kernels become L1/TEX-bound.  So global memory is only ever touched in "chunk layout": lane
 // l holds the 16-byte pieces j*32+l (j = 0..3) of the chunk, i.e. fully coalesced 128-bit accesses.
 // Element-wise work (axpy, dots, norms) is done directly in chunk layout; only stencils and the block
 // preconditioner need row layout, and the two layouts are converted through a per-warp shared-memory
@@ -268,10 +267,10 @@ __device__ __forceinline__ void rows_lap(const double *__restrict__ z, int row0,
   chunk_ld(z, row0, nvalid, lane, cz);
   rows_lap_c(cz, z, row0, nvalid, nbr, sw, lane, c, out, irr);
 }
-// ---- rows_lap_coop: the variant the SpMV kernels use (measured there: 0.291 vs 0.302 ms at 8192^2; k_init and the
-// right-hand-side kernel, with their higher register pressure, are 4 % faster on the plain form below, profiles/r02k) ----
-// The L1 data pipe (shared-memory and global-load wavefronts together) is what bounds the stencil kernels, not DRAM
-// (profiles/r02i_krylov_ncu.md: 75 % against 70 %), and the neighbour accesses were 60 % of its global part.  So:
+// ---- rows_lap_coop: the variant the SpMV kernels use (k_init and the right-hand-side kernel, with their higher register
+// pressure, keep the plain form below) ----
+// The L1 data pipe (shared-memory and global-load wavefronts together) bounds the stencil kernels about as much as DRAM
+// does, and the neighbour accesses are most of its global part.  So:
 //  * the edge rows of the S/N neighbour blocks come in with ONE warp-wide 128-bit load: lanes 0..15 fetch the four 16-byte
 //    pieces of row 0 of the N neighbour of each of the warp's four blocks, lanes 16..31 row 7 of the S neighbours (8 wavefronts
 //    instead of 32 for eight quarter-empty per-lane loads); the pieces are staged behind the chunk in the scratch;

@@ -1,4 +1,4 @@
-// LocalSpMatDnVec on the B200 hot path: link THIS object (+ libcup2d_b200.so) instead of the reference's
+// LocalSpMatDnVec on the cup2d_b200 hot path: link THIS object (+ libcup2d_b200.so) instead of the reference's
 // cuda.o and the unmodified main.cpp runs its pressure solves through cup2d_b200.
 //
 // It implements the class exactly as the reference declares it (cuda.h:26-79 is included from the

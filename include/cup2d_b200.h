@@ -1,11 +1,11 @@
-/* cup2d_b200 — C ABI of the B200-native CUP2D hot path (libcup2d_b200.so).
+/* cup2d_b200 — C ABI of the CUDA-native (H100, sm_90a) CUP2D hot path (libcup2d_b200.so).
  *
  * Plain pointers and sizes only; no C++/torch types cross this boundary.  Every entry point
  * returns 0 on success and a negative CUP2D_E* code on failure; cup2d_last_error() gives the
  * message (the reference itself has no error convention: CUDA errors are swallowed, cuda.cu:358;
  * this library fails loudly instead).
  *
- * What each group replaces in the reference (/root/reference, file:line):
+ * What each group replaces in the reference (slitvinov/CUP2D, file:line):
  *   grid / fields   Grid, Info, var.{vel,vold,tmpV,chi,pres,pold,tmp}     main.cpp:504-512, 2193-2201, 3264-3278, 6508-6541
  *   compute_dt      umax reduction + dt rule                              main.cpp:6579-6595
  *   advect_diffuse  computeA<VectorLab>(KernelAdvectDiffuse) + RK2 loops  main.cpp:5441-5503, 6607-6642, 162-208
@@ -33,7 +33,7 @@ enum {
   CUP2D_OK = 0,
   CUP2D_EINVAL = -1,  /* bad argument / unsupported topology */
   CUP2D_ECUDA = -2,   /* CUDA runtime error (message in cup2d_last_error) */
-  CUP2D_ENOGPU = -3,  /* no usable sm_100 device: there is NO CPU fallback */
+  CUP2D_ENOGPU = -3,  /* no usable sm_90 device: there is NO CPU fallback */
   CUP2D_ESTATE = -4,  /* call made in the wrong state (e.g. multi-rank step before peers attached) */
   CUP2D_ECOMM = -5    /* a cross-GPU wait ran into its time limit (peer dead, or ranks issued different call sequences);
                          the reference aborts through MPI in that situation (SURVEY.md 8(b) error convention) */
@@ -269,8 +269,7 @@ int64_t cup2d_amr_plan_poisson(cup2d_amr_plan *p, int32_t *nbr_out, int64_t *nnz
 int64_t cup2d_amr_plan_faces(cup2d_amr_plan *p, int32_t *out);
 
 /* ---- multi-level meshes on the device: first, correctness-oriented path (csrc/amr_ops.cu) --------------------------
- * NOT YET VALIDATED ON HARDWARE (written after round 1's GPU budget was spent; tests/test_gpu_amr.py runs only with
- * CUP2D_TEST_UNVALIDATED=1).  One GPU.  Same field ids and block layout as the uniform-grid context, blocks in `infos` order. */
+ * Checked on the GPU by tests/test_gpu_amr.py.  One GPU.  Same field ids and block layout as the uniform-grid context, blocks in `infos` order. */
 typedef struct cup2d_amr cup2d_amr;
 int cup2d_amr_create(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, double h0, double nu,
                      int32_t device, cup2d_amr **out);

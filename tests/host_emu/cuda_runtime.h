@@ -7,7 +7,7 @@
 #include <cstdint>
 #include <cstdio>
 
-struct cudaDeviceProp { int major = 10, minor = 0, multiProcessorCount = 4; char name[64] = "host emulation (sm_100 semantics)"; };
+struct cudaDeviceProp { int major = 9, minor = 0, multiProcessorCount = 4; char name[64] = "host emulation (sm_90 semantics)"; };
 inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { *p = cudaDeviceProp(); return 0; }
 typedef struct EmuEvent *cudaEvent_t;
 inline cudaError_t cudaEventCreate(cudaEvent_t *e) { *e = nullptr; return 0; }

@@ -357,7 +357,7 @@ assert worst < 1e-11
 
 # The two sanitizer builds recompile every product source with -fsanitize and take 4-6 minutes on 8 cores: they run when asked
 # for (CUP2D_TEST_SANITIZERS=1, as tools/run_emulated_gpu_tests.sh does); the hardware counterpart is compute-sanitizer
-# memcheck/racecheck on the GPU box (profiles/r02a_sanitizer_*).
+# memcheck/racecheck on a GPU.
 sanitizers = pytest.mark.skipif(os.environ.get("CUP2D_TEST_SANITIZERS") != "1", reason="sanitizer builds are opt-in: CUP2D_TEST_SANITIZERS=1")
 
 
@@ -414,8 +414,7 @@ def test_measurement_variants_keep_parity():
     """the build switches of the advect stage that are OFF in the default build (advect.cu: CUP2D_ADV_LDGSTS=0 — the tile
     filled by per-row bulk copies on one mbarrier instead of cp.async; CUP2D_ADV_SPECIALIZE=0 — one copy of the line code with
     run-time strides for both passes; CUP2D_ADV_FASTPATH=0 — every line through the general core) built together into an
-    emulated library: the operator / advect / time-step parity tests still pass.  (Each was also run on hardware:
-    profiles/r02e_variants.jsonl, r02g_variants.jsonl.)"""
+    emulated library: the operator / advect / time-step parity tests still pass."""
     sys.path.insert(0, os.path.join(HERE, "host_emu"))
     import build
     lib = build.build_full(("CUP2D_ADV_LDGSTS=0", "CUP2D_ADV_SPECIALIZE=0", "CUP2D_ADV_FASTPATH=0"), "_variants")
@@ -454,53 +453,40 @@ def test_reference_time_loop_on_the_emulated_library(emulated_library, golden_di
     assert np.abs(f[:, 2] - g["p"]).max() < 1e-10
 
 
-def test_reference_loop_with_bodies_device_resident_on_the_emulated_library(emulated_library, tmp_path):
+def test_reference_loop_with_bodies_device_resident_on_the_emulated_library(emulated_library, golden_dir, tmp_path):
     """the device-resident form of the drop-in, WITH bodies: the reference's own loop with RK2, the penalisation sums, the
     blend, the u_def assembly and the pressure section on the library (dropin/resident_*.inc over main.cpp:6607-6642, 6648-6679,
     6945-6979, 6981-7187) while ongrid(), the 3x3 rigid-motion solve, the collision model and the forces stay on the host —
-    two interacting fish, 4 steps (the last one with a collision), against the unmodified reference run the same way"""
+    two interacting fish, 4 steps (the last one with a collision), against the unmodified reference run the same way
+    (tests/golden/driver_fsteps_L4_k5.npz: u, v, p at its sample of cells, dt and the body states in full)"""
     import numpy as np
     if not os.path.exists("/root/reference/main.cpp"):
         pytest.skip("needs the reference sources to build the patched driver (build container only)")
     emu_dir = os.path.dirname(emulated_library)
-    subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref", "ref_resident", f"LIBDIR={emu_dir}", "LIBNAME=cup2d_emu",
+    subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref_resident", f"LIBDIR={emu_dir}", "LIBNAME=cup2d_emu",
                     "RESIDENT=ref_harness_resident_emu", f"RPATH={emu_dir}"], check=True, stdout=subprocess.DEVNULL)
-    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER="5",
+    g = np.load(os.path.join(golden_dir, "driver_fsteps_L4_k5.npz"))
+    L, K, ns = int(g["L"]), int(g["kiter"]), len(g["dt"])
+    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER=str(K),
                CUP2D_REF_SHAPES="angle=0 L=0.8 xpos=0.52 ypos=0.44\n angle=175 L=0.8 xpos=0.47 ypos=0.56")
-    outs = []
-    for exe in ("ref_harness", "ref_harness_resident_emu"):
-        out = tmp_path / (exe + ".bin")
-        subprocess.run([os.path.join(ROOT, "oracle", "_ref", exe), "fsteps", "4", "4", "5", str(out)], check=True,
-                       stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL, env=env, timeout=900)
-        outs.append(np.fromfile(out))
-    N = 128
-    a, b = (o.reshape(-1, 1 + 3 * N * N + 10) for o in outs)
-    assert a.shape == b.shape and len(a) == 4
-    assert np.abs(a[:, 0] - b[:, 0]).max() < 1e-15                      # dt
-    assert np.abs(a[:, 1:-10] - b[:, 1:-10]).max() < 1e-12              # u, v, p
-    assert np.abs(a[:, -10:] - b[:, -10:]).max() < 1e-12                # centre of mass, u, v, omega of both fish
-    assert np.abs(a[-1, 1:1 + N * N]).max() > 0.1                       # the fish really drive the flow
-
-
-def _parse_asteps(path):
-    import numpy as np
-    a, i, out = np.fromfile(path), 0, []
-    while i < len(a):
-        dt, nb = a[i], int(a[i + 1])
-        i += 2
-        mesh = a[i:i + 3 * nb].reshape(nb, 3).astype(int)
-        i += 3 * nb
-        vel, pres = a[i:i + 128 * nb], a[i + 128 * nb:i + 192 * nb]
-        i += 192 * nb
-        out.append((dt, mesh, vel, pres))
-    return out
+    out = tmp_path / "resident.bin"
+    subprocess.run([os.path.join(ROOT, "oracle", "_ref", "ref_harness_resident_emu"), "fsteps", str(L), str(ns), str(K), str(out)],
+                   check=True, stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL, env=env, timeout=900)
+    N = 8 << L
+    b = np.fromfile(out).reshape(-1, 1 + 3 * N * N + 10)
+    assert len(b) == ns == 4
+    assert np.abs(b[:, 0] - g["dt"]).max() < 1e-15                                      # dt
+    assert np.abs(b[:, 1:-10][:, g["fields_idx"]] - g["fields"]).max() < 1e-12          # u, v, p
+    assert np.abs(b[:, -10:] - g["bodies"]).max() < 1e-12                               # centre of mass, u, v, omega of both fish
+    assert g["u_absmax"][-1] > 0.1 and np.abs(b[-1, 1:1 + N * N]).max() > 0.1          # the fish really drive the flow
 
 
 @pytest.mark.parametrize("form,steps", [("amrloop", 2), ("amrresident", 3)])
-def test_reference_amr_case_on_the_multi_level_path_emulated(emulated_library, tmp_path, form, steps):
+def test_reference_amr_case_on_the_multi_level_path_emulated(emulated_library, golden_dir, tmp_path, form, steps):
     """config C1 end to end: the reference's own run.sh case (two fish, 7 refinement levels, 278 blocks, its own adapt() /
     ongrid() on the host) on the multi-level path of the library (fast kernels, Poisson rows from the library's own plan),
-    linked against the emulated library, against the unmodified reference: same mesh and fields to rounding at every step.
+    linked against the emulated library, against the unmodified reference (tests/golden/driver_asteps_lmax8_k5.npz): same mesh
+    and fields to rounding at every step.
       amrloop      RK2 and the whole pressure section on cup2d_amr, penalisation on the host (dropin/amr_loop_*.inc)
       amrresident  additionally the penalisation sums, the blend and the u_def assembly on the device
                    (cup2d_amr_shape_*, dropin/amr_resident_*.inc): the velocity crosses PCIe once each way per step
@@ -510,20 +496,23 @@ def test_reference_amr_case_on_the_multi_level_path_emulated(emulated_library, t
     if not os.path.exists("/root/reference/main.cpp"):
         pytest.skip("needs the reference sources to build the patched driver (build container only)")
     emu_dir = os.path.dirname(emulated_library)
-    subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), "ref", f"ref_{form}", f"LIBDIR={emu_dir}", "LIBNAME=cup2d_emu",
+    subprocess.run(["make", "-C", os.path.join(ROOT, "oracle"), f"ref_{form}", f"LIBDIR={emu_dir}", "LIBNAME=cup2d_emu",
                     f"{form.upper()}=ref_harness_{form}_emu", f"RPATH={emu_dir}"], check=True, stdout=subprocess.DEVNULL)
+    sys.path.insert(0, golden_dir)
+    from make_driver_golden import parse_asteps
+    g = np.load(os.path.join(golden_dir, "driver_asteps_lmax8_k5.npz"))   # 3 steps: the first `steps` of them are compared
+    K = int(g["kiter"])
     # amrresident also takes adapt()'s tagging field from the device (cup2d_amr_adapt_tags, eleven adapt() calls in this
     # short run, the initial refinement included): the mesh must be the reference's from the start
-    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER="5", CUP2D_B200_AMR_FAST="1", CUP2D_B200_AMR_TAGS="1")
-    runs = []
-    for exe in ("ref_harness", f"ref_harness_{form}_emu"):
-        out = tmp_path / (exe + ".bin")
-        subprocess.run([os.path.join(ROOT, "oracle", "_ref", exe), "asteps", "8", str(steps), "5", str(out)], check=True,
-                       stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL, env=env, timeout=1500)
-        runs.append(_parse_asteps(out))
-    assert len(runs[0]) == len(runs[1]) == steps
-    for (dt0, m0, v0, p0), (dt1, m1, v1, p1) in zip(*runs):
-        assert m0.shape == m1.shape and (m0 == m1).all() and len(set(m0[:, 0].tolist())) >= 5
-        assert abs(dt0 - dt1) < 1e-15
-        assert np.abs(v0 - v1).max() < 1e-12 * np.abs(v0).max()
-        assert np.abs(p0 - p1).max() < 1e-11 * max(np.abs(p0).max(), 1e-300)
+    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER=str(K), CUP2D_B200_AMR_FAST="1", CUP2D_B200_AMR_TAGS="1")
+    out = tmp_path / "asteps.bin"
+    subprocess.run([os.path.join(ROOT, "oracle", "_ref", f"ref_harness_{form}_emu"), "asteps", str(int(g["level_max"])), str(steps),
+                    str(K), str(out)], check=True, stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL, env=env, timeout=1500)
+    run = parse_asteps(out)
+    assert len(run) == steps <= int(g["nsteps"])
+    for s, (dt, mesh, vel, pres) in enumerate(run):
+        m0 = g[f"mesh_{s}"]
+        assert mesh.shape == m0.shape and (mesh == m0).all() and len(set(m0[:, 0].tolist())) >= 5
+        assert abs(dt - g[f"dt_{s}"]) < 1e-15
+        assert np.abs(vel[g[f"vel_idx_{s}"]] - g[f"vel_{s}"]).max() < 1e-12 * g[f"vel_absmax_{s}"]
+        assert np.abs(pres[g[f"pres_idx_{s}"]] - g[f"pres_{s}"]).max() < 1e-11 * max(g[f"pres_absmax_{s}"], 1e-300)

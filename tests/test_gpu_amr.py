@@ -3,8 +3,7 @@ tagging of cup2d_amr_adapt_tags) against the reference's own outputs on its 7-le
 amrtags_lmax8.npz), against the reference restatement on a second mesh family, and in situ (the reference's run.sh case
 with its hot path spliced onto this path).
 
-First run on hardware in round 2 (profiles/r02a_first_contact.md: all green on a B200, compute-sanitizer memcheck and
-racecheck clean); they also pass on the CPU against the emulated build of the same sources
+They also pass on the CPU against the emulated build of the same sources
 (tools/run_emulated_gpu_tests.sh, tests/test_full_emulation.py)."""
 import os
 
@@ -320,31 +319,31 @@ def test_amr_bodies_sums_blend_and_udef_assembly(case):
 
 
 @pytest.mark.parametrize("form", ["amrloop", "amrresident"])
-def test_reference_amr_case_on_the_multi_level_device_path(tmp_path, form):
+def test_reference_amr_case_on_the_multi_level_device_path(golden_dir, tmp_path, form):
     """config C1 on the device: the reference's own run.sh case with RK2 and the pressure section on cup2d_amr (fast kernels)
     — oracle/_ref/ref_harness_amrloop; with the penalisation sums, blend and u_def assembly there too: ..._amrresident —
-    against the unmodified reference loop (oracle/_ref/ref_harness), 6 steps"""
+    against the unmodified reference loop (tests/golden/driver_asteps_lmax8_k8.npz, recorded from oracle/_ref/ref_harness),
+    6 steps: dt and mesh in full, velocity and pressure at the golden's sample of entries"""
     import subprocess
+    import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exes = [os.path.join(root, "oracle", "_ref", n) for n in ("ref_harness", f"ref_harness_{form}")]
-    if not all(os.path.exists(e) for e in exes):
-        pytest.skip("oracle/_ref binaries not built")
-    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER="8", CUP2D_B200_AMR_FAST="1")
-    runs = []
-    for exe in exes:
-        out = tmp_path / (os.path.basename(exe) + ".bin")
-        subprocess.run([exe, "asteps", "8", "6", "8", str(out)], check=True, stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL,
-                       env=env, timeout=600)
-        a, i, steps = np.fromfile(out), 0, []
-        while i < len(a):
-            dt, nb = a[i], int(a[i + 1])
-            steps.append((dt, a[i + 2:i + 2 + 3 * nb].copy(), a[i + 2 + 3 * nb:i + 2 + 131 * nb].copy(), a[i + 2 + 131 * nb:i + 2 + 195 * nb].copy()))
-            i += 2 + 195 * nb
-        runs.append(steps)
-    assert len(runs[0]) == len(runs[1]) == 6
-    for (dt0, m0, v0, p0), (dt1, m1, v1, p1) in zip(*runs):
-        assert np.array_equal(m0, m1) and abs(dt0 - dt1) < 1e-14
-        assert np.abs(v0 - v1).max() < 1e-10 * np.abs(v0).max() and np.abs(p0 - p1).max() < 1e-9 * np.abs(p0).max()
+    exe = os.path.join(root, "oracle", "_ref", f"ref_harness_{form}")
+    if not os.path.exists(exe):
+        pytest.skip(f"oracle/_ref/ref_harness_{form} not built (make -C oracle all: needs the reference sources)")
+    sys.path.insert(0, golden_dir)
+    from make_driver_golden import parse_asteps
+    g = np.load(os.path.join(golden_dir, "driver_asteps_lmax8_k8.npz"))
+    ns, K = int(g["nsteps"]), int(g["kiter"])
+    env = dict(os.environ, OMP_NUM_THREADS="1", CUP2D_B200_MAX_ITER=str(K), CUP2D_B200_AMR_FAST="1")
+    out = tmp_path / "asteps.bin"
+    subprocess.run([exe, "asteps", str(int(g["level_max"])), str(ns), str(K), str(out)], check=True, stderr=subprocess.DEVNULL,
+                   stdout=subprocess.DEVNULL, env=env, timeout=600)
+    steps = parse_asteps(out)
+    assert len(steps) == ns == 6
+    for s, (dt, mesh, vel, pres) in enumerate(steps):
+        assert np.array_equal(mesh, g[f"mesh_{s}"]) and abs(dt - g[f"dt_{s}"]) < 1e-14
+        assert np.abs(vel[g[f"vel_idx_{s}"]] - g[f"vel_{s}"]).max() < 1e-10 * g[f"vel_absmax_{s}"]
+        assert np.abs(pres[g[f"pres_idx_{s}"]] - g[f"pres_{s}"]).max() < 1e-9 * g[f"pres_absmax_{s}"]
 
 
 def test_two_ranks_on_two_gpus_multi_level():

@@ -263,35 +263,30 @@ def test_large_grid_properties():
     sim.close()
 
 
-def test_reference_driver_with_adapter_matches_reference_gpu_solver(tmp_path):
+def test_reference_driver_with_adapter_matches_reference_gpu_solver(golden_dir, tmp_path):
     """The drop-in boundary: the UNMODIFIED reference time loop linked against
     dropin/local_spmat_adapter.cpp + libcup2d_b200.so (oracle/_ref/ref_harness_b200) against the same loop
-    with the reference's own cuda.cu (oracle/_ref/ref_harness_gpu): 1 step, 1000 iterations."""
+    with the reference's own cuda.cu (tests/golden/driver_gpu_steps_L3.npz, recorded from oracle/_ref/ref_harness_gpu by
+    tests/golden/make_driver_golden.py): 1 step, 1000 iterations."""
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    bins = [os.path.join(root, "oracle", "_ref", n) for n in ("ref_harness_gpu", "ref_harness_b200")]
-    if not all(os.path.exists(b) for b in bins):
-        pytest.skip("oracle/_ref binaries not built (make -C oracle all in the build container)")
-    L = 3
+    exe = os.path.join(root, "oracle", "_ref", "ref_harness_b200")
+    if not os.path.exists(exe):
+        pytest.skip("oracle/_ref/ref_harness_b200 not built (make -C oracle all: needs the reference sources)")
+    g = np.load(os.path.join(golden_dir, "driver_gpu_steps_L3.npz"))
+    L = int(g["L"])
     N = 8 << L
-    u, v, p, *_ = make_fields(N, 77)
+    u, v, p, *_ = make_fields(N, int(g["seed"]))
     z = np.zeros((N, N))
-    fin = tmp_path / "in.bin"
+    fin, fout = tmp_path / "in.bin", tmp_path / "out.bin"
     np.concatenate([a.ravel() for a in (u, v, p, z, z, z)]).tofile(fin)
-    outs = []
-    for b in bins:
-        fout = tmp_path / (os.path.basename(b) + ".bin")
-        try:
-            subprocess.run([b, "steps", str(L), "1e-3", "0.5", "1", "1000", str(fin), str(fout)], check=True,
-                           stderr=subprocess.DEVNULL, env=dict(os.environ, OMP_NUM_THREADS="8"), timeout=420)
-        except subprocess.TimeoutExpired:
-            pytest.skip(f"{os.path.basename(b)} did not finish in 420 s (cold cuBLAS/cuSPARSE load on this box); "
-                        "the comparison is recorded in profiles/README.md section 3")
-        outs.append(np.fromfile(fout).reshape(1, 1 + 5 * N * N))
-    assert np.abs(outs[0][:, 0] - outs[1][:, 0]).max() < 1e-14          # dt
-    f0, f1 = outs[0][:, 1:].reshape(1, 5, N, N), outs[1][:, 1:].reshape(1, 5, N, N)
+    subprocess.run([exe, "steps", str(L), "1e-3", "0.5", "1", str(int(g["kiter"])), str(fin), str(fout)], check=True,
+                   stderr=subprocess.DEVNULL, env=dict(os.environ, OMP_NUM_THREADS="8"), timeout=420)
+    out = np.fromfile(fout).reshape(1, 1 + 5 * N * N)
+    assert np.abs(out[:, 0] - g["dt"]).max() < 1e-14          # dt
+    f = out[:, 1:].reshape(1, 5, N, N)
     # contract: L-inf(u,v,p) < 1e-6; observed ~1e-12 (u,v) / 1e-10 (p) after 1000 Krylov iterations
-    assert np.abs(f0[:, :3] - f1[:, :3]).max() < 1e-8
+    assert max(np.abs(f[:, 0] - g["u"]).max(), np.abs(f[:, 1] - g["v"]).max(), np.abs(f[:, 2] - g["p"]).max()) < 1e-8
 
 
 @pytest.mark.parametrize("name", ["steps_L2_random_k8", "steps_L3_tg_k15"])
@@ -323,32 +318,29 @@ def test_reference_driver_patched_loop_matches_golden(golden_dir, name, tmp_path
     assert np.abs(f[:, 2] - g["p"]).max() < 1e-10
 
 
-def test_reference_driver_resident_loop_with_bodies(tmp_path):
+def test_reference_driver_resident_loop_with_bodies(golden_dir, tmp_path):
     """The device-resident drop-in with bodies (oracle/_ref/ref_harness_resident: dropin/resident_*.inc spliced over
     main.cpp:6607-6642, 6648-6679, 6945-6979, 6981-7187) against the unmodified reference loop with its CPU solver
-    (oracle/_ref/ref_harness): two interacting fish, 4 steps, 8 Poisson iterations each."""
+    (tests/golden/driver_fsteps_L4_k8.npz, recorded from oracle/_ref/ref_harness): two interacting fish, 4 steps, 8 Poisson
+    iterations each; u, v, p at the golden's sample of cells, dt and the body states in full."""
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exes = [os.path.join(root, "oracle", "_ref", n) for n in ("ref_harness", "ref_harness_resident")]
-    if not all(os.path.exists(e) for e in exes):
-        pytest.skip("oracle/_ref binaries not built (make -C oracle all in the build container)")
-    env = dict(os.environ, OMP_NUM_THREADS="8", CUP2D_B200_MAX_ITER="8",
+    exe = os.path.join(root, "oracle", "_ref", "ref_harness_resident")
+    if not os.path.exists(exe):
+        pytest.skip("oracle/_ref/ref_harness_resident not built (make -C oracle all: needs the reference sources)")
+    g = np.load(os.path.join(golden_dir, "driver_fsteps_L4_k8.npz"))
+    L, K, ns = int(g["L"]), int(g["kiter"]), len(g["dt"])
+    env = dict(os.environ, OMP_NUM_THREADS="8", CUP2D_B200_MAX_ITER=str(K),
                CUP2D_REF_SHAPES="angle=0 L=0.8 xpos=0.52 ypos=0.44\n angle=175 L=0.8 xpos=0.47 ypos=0.56")
-    outs = []
-    for exe in exes:
-        out = tmp_path / (os.path.basename(exe) + ".bin")
-        try:
-            subprocess.run([exe, "fsteps", "4", "4", "8", str(out)], check=True, stderr=subprocess.DEVNULL, stdout=subprocess.DEVNULL,
-                           env=env, timeout=300)
-        except subprocess.TimeoutExpired:
-            pytest.skip("a reference driver did not finish in 300 s on this box")
-        outs.append(np.fromfile(out))
-    N = 128
-    a, b = (o.reshape(-1, 1 + 3 * N * N + 10) for o in outs)
-    assert a.shape == b.shape and len(a) == 4
-    assert np.abs(a[:, 0] - b[:, 0]).max() < 1e-14
-    assert np.abs(a[:, 1:-10] - b[:, 1:-10]).max() < 1e-9    # OpenMP summation order on the reference side
-    assert np.abs(a[:, -10:] - b[:, -10:]).max() < 1e-9
+    out = tmp_path / "resident.bin"
+    subprocess.run([exe, "fsteps", str(L), str(ns), str(K), str(out)], check=True, stderr=subprocess.DEVNULL,
+                   stdout=subprocess.DEVNULL, env=env, timeout=300)
+    N = 8 << L
+    b = np.fromfile(out).reshape(-1, 1 + 3 * N * N + 10)
+    assert len(b) == ns == 4
+    assert np.abs(b[:, 0] - g["dt"]).max() < 1e-14
+    assert np.abs(b[:, 1:-10][:, g["fields_idx"]] - g["fields"]).max() < 1e-9    # OpenMP summation order on the reference side
+    assert np.abs(b[:, -10:] - g["bodies"]).max() < 1e-9
 
 
 def test_rectangular_domain_vs_reference_golden(golden_dir):
@@ -377,32 +369,39 @@ def test_rectangular_domain_vs_reference_golden(golden_dir):
     sim.close()
 
 
-def test_reference_amr_case_through_adapter():
+def test_reference_amr_case_through_adapter(golden_dir, tmp_path):
     """SURVEY §8(f) rank 1: the reference's own run.sh case (2 fish, block-AMR) with its pressure solves on
     cup2d_b200 through the LocalSpMatDnVec adapter (coarse-fine rows via the CSR side table) against the same
-    driver with the reference's cuda.cu.  Same grid every step; solutions within the 1e-6 contract."""
+    driver with the reference's cuda.cu (tests/golden/driver_gpu_amr_lmax8.npz, recorded from oracle/_ref/ref_harness_gpu).
+    Same grid every step; solutions within the 1e-6 contract."""
+    import subprocess
     import sys
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    if not all(os.path.exists(os.path.join(root, "oracle", "_ref", n)) for n in ("ref_harness_gpu", "ref_harness_b200")):
-        pytest.skip("oracle/_ref binaries not built")
+    exe = os.path.join(root, "oracle", "_ref", "ref_harness_b200")
+    if not os.path.exists(exe):
+        pytest.skip("oracle/_ref/ref_harness_b200 not built (make -C oracle all: needs the reference sources)")
     sys.path.insert(0, os.path.join(root, "tools"))
-    import ref_gpu_compare_amr as cmp
-    import subprocess
-    try:
-        res = cmp.compare(nsteps=2, timeout=420)
-    except subprocess.TimeoutExpired:
-        pytest.skip("the reference's GPU binary did not finish in 420 s (cold cuBLAS/cuSPARSE load on this box); "
-                    "the comparison is recorded in profiles/r01i_amr_compare.json")
-    assert len(res["steps"]) == 2
-    for row in res["steps"]:
-        assert row["same_grid"] and len(row["levels"]) >= 2     # really multi-level
-        assert row["dt_diff"] < 1e-7
-        assert row["b_Linf"] < 1e-6 * max(1.0, row["b_scale"])
-        # mean-free solution (the constant mode of the singular system is free).  With tolerance 0 both solvers run 1000
-        # iterations on a residual that reaches round-off level after a few hundred and return the best iterate of a noisy
-        # plateau, picked by different rounding: 2e-8 ... 1.2e-6 over the runs of two rounds (profiles/README.md), the size
-        # of the difference between cuda.cu and its own CPU restatement (tools/ref_gpu_compare.py)
-        assert row["x_Linf"] < 1e-5 * max(1.0, row["x_scale"])
+    from ref_gpu_compare_amr import read_records
+    g = np.load(os.path.join(golden_dir, "driver_gpu_amr_lmax8.npz"))
+    ns = int(g["nsteps"])
+    out = tmp_path / "amr.bin"
+    subprocess.run([exe, "amr", str(int(g["level_max"])), str(ns), str(int(g["kiter"])), str(out)], check=True,
+                   stderr=subprocess.DEVNULL, env=dict(os.environ, OMP_NUM_THREADS="8"), timeout=420)
+    recs = read_records(out)
+    assert len(recs) == ns == 2
+    for s, r in enumerate(recs):
+        lij = g[f"lij_{s}"]
+        assert r["lij"].shape == lij.shape and (r["lij"] == lij).all() and len(set(lij[:, 0].tolist())) >= 2  # really multi-level
+        assert abs(r["dt"] - g[f"dt_{s}"]) < 1e-7
+        assert np.abs(r["b"] - g[f"b_{s}"]).max() < 1e-6 * max(1.0, np.abs(g[f"b_{s}"]).max())
+        # mean-free solution (the constant mode of the singular system is free; the driver removes the volume-weighted mean,
+        # main.cpp:7126-7148).  With tolerance 0 both solvers run 1000 iterations on a residual that reaches round-off level
+        # after a few hundred and return the best iterate of a noisy plateau, picked by different rounding: up to ~1e-6, the
+        # size of the difference between cuda.cu and its own CPU restatement (tools/ref_gpu_compare.py)
+        w = np.repeat(4.0 ** (-lij[:, 0].astype(np.float64)), 64)
+        xa = g[f"x_{s}"] - (w * g[f"x_{s}"]).sum() / w.sum()
+        xb = r["x"] - (w * r["x"]).sum() / w.sum()
+        assert np.abs(xa - xb).max() < 1e-5 * max(1.0, np.abs(xa).max())
 
 
 def test_two_ranks_on_two_gpus_match_the_oracle():

@@ -1,4 +1,4 @@
-"""BASELINE.json configs[2]-style measurement: 4096^2 uniform grid on one B200, time steps whose Poisson solves stop on the
+"""BASELINE.json configs[2]-style measurement: 4096^2 uniform grid on one GPU, time steps whose Poisson solves stop on the
 tolerance (poissonTol 1e-6; stopping rule cuda.cu:535-541, main.cpp:7028-7030) instead of after a fixed iteration count.
 
 The whole step — dt control, RK2, right-hand side, the BiCGSTAB loop as a graph WHILE node whose condition the device sets,
