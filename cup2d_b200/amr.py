@@ -7,7 +7,25 @@ import numpy as np
 
 from . import lib as _l
 
-LAB_SHAPES = {0: (14, 14, 2), 1: (10, 10, 2), 2: (10, 10, 1), 3: (16, 16, 1)}  # kind 3: chi lab of GradChiOnTmp
+LAB_SHAPES = {0: (14, 14, 2), 1: (10, 10, 2), 2: (10, 10, 1), 3: (16, 16, 1),  # kind 3: chi lab of GradChiOnTmp
+              4: (10, 10, 2), 5: (10, 10, 1)}  # kinds 4, 5: the +-1 labs with corners that adapt() refines from
+
+
+def adapt_mesh(blocks, bpdx, bpdy, level_max, block_linf, rtol, ctol):
+    """adapt()'s refine / compress decision (cup2d_amr_adapt_mesh, host only): the block list after one adapt() of the mesh
+    `blocks` with the per-block L-inf `block_linf` of the tagging field, in the reference's order"""
+    lib = _l.load_library()
+    b = np.ascontiguousarray(blocks, dtype=np.int32).reshape(-1, 3)
+    linf = np.ascontiguousarray(block_linf, dtype=np.float64)
+    assert len(linf) == len(b)
+    args = (len(b), b.ctypes.data_as(C.POINTER(C.c_int32)), int(bpdx), int(bpdy), int(level_max),
+            linf.ctypes.data_as(C.POINTER(C.c_double)), float(rtol), float(ctol))
+    n = lib.cup2d_amr_adapt_mesh(*args, None)
+    if n < 0:
+        _l.check(int(n))
+    out = np.empty((n, 3), dtype=np.int32)
+    lib.cup2d_amr_adapt_mesh(*args, out.ctypes.data_as(C.POINTER(C.c_int32)))
+    return out
 
 
 class AmrPlan:
@@ -100,6 +118,7 @@ class AmrSimulation:
     def __init__(self, level_ij, bpdx, bpdy, h0, nu, device=0):
         self.lib = _l.load_library()
         self.blocks = np.ascontiguousarray(level_ij, dtype=np.int32).reshape(-1, 3)
+        self.bpdx, self.bpdy = int(bpdx), int(bpdy)
         self._h = C.c_void_p()
         _l.check(self.lib.cup2d_amr_create(len(self.blocks), self.blocks.ctypes.data_as(C.POINTER(C.c_int32)), bpdx, bpdy,
                                            float(h0), float(nu), device, C.byref(self._h)))
@@ -114,6 +133,7 @@ class AmrSimulation:
         rb = np.ascontiguousarray(rank_begin, dtype=np.int64)
         nranks = len(rb) - 1
         self.blocks = allb[int(rb[rank]):int(rb[rank + 1])]
+        self.bpdx, self.bpdy = int(bpdx), int(bpdy)
         self._h = C.c_void_p()
         _l.check(self.lib.cup2d_amr_create_ranks(len(allb), allb.ctypes.data_as(C.POINTER(C.c_int32)), bpdx, bpdy, float(h0), float(nu),
                                                  int(rank), nranks, rb.ctypes.data_as(C.POINTER(C.c_int64)), device, C.byref(self._h)))
@@ -214,6 +234,22 @@ class AmrSimulation:
         out = np.empty(len(self.blocks))
         _l.check(self.lib.cup2d_amr_adapt_tags(self._h, float(rtol), int(level_max), out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
+
+    def regrid(self, new_blocks):
+        """move the context onto `new_blocks` (one refine / compress step away, e.g. from adapt_mesh) with adapt()'s field
+        transfer on the device (cup2d_amr_regrid); tmpV is zero afterwards and the shapes have to be set again"""
+        b = np.ascontiguousarray(new_blocks, dtype=np.int32).reshape(-1, 3)
+        _l.check(self.lib.cup2d_amr_regrid(self._h, len(b), b.ctypes.data_as(C.POINTER(C.c_int32))))
+        self.blocks = b.copy()
+
+    def adapt(self, rtol, ctol, level_max):
+        """adapt() on the device-resident fields: tags -> decision -> regrid; returns whether the mesh changed"""
+        linf = self.adapt_tags(rtol, level_max)
+        new = adapt_mesh(self.blocks, self.bpdx, self.bpdy, level_max, linf, rtol, ctol)
+        if np.array_equal(new, self.blocks):
+            return False
+        self.regrid(new)
+        return True
 
     # ---- bodies (cup2d_amr_shape_*): the calls of Simulation.shape_* on the multi-level context ----
     def shape_set(self, shape, ids, X, udef):

@@ -12,6 +12,8 @@ void cup2d_amr_plan_destroy(cup2d_amr_plan *p);
 int64_t cup2d_amr_plan_stencil(cup2d_amr_plan *p, int which, int64_t *rowptr, int32_t *src_block, int32_t *src_cellcomp,
                                double *weight);
 int64_t cup2d_amr_plan_faces(cup2d_amr_plan *p, int32_t *out);
+int cup2d_amr_create(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, double h0, double nu,
+                     int32_t device, cup2d_amr **out);
 int64_t cup2d_amr_plan_poisson(cup2d_amr_plan *p, int32_t *nbr_out, int64_t *nnz_out, int32_t *irr_rows, int32_t *irr_rowptr,
                                int32_t *irr_col, double *irr_val);
 int cup2d_amr_advect_diffuse_rhs(cup2d_amr *a, double dt);
@@ -49,6 +51,12 @@ struct CoarseFace { // one coarse-fine face seen from the coarse side
 };
 
 } // namespace cup2d
+
+// the plan's block list, [n][3] (level, i, j), and its level-0 blocks per direction
+const std::vector<int> &amr_plan_level_ij(const cup2d_amr_plan *p, int *bpdx, int *bpdy);
+// full lab rows (as cup2d_amr_plan_stencil) of the blocks `blocks[0..nsub)` only, in that order (csrc/amr_regrid.cu)
+int amr_plan_subset_rows(cup2d_amr_plan *p, int which, int64_t nsub, const int32_t *blocks, std::vector<int64_t> &rowptr,
+                         std::vector<int32_t> &src_block, std::vector<int32_t> &src_cellcomp, std::vector<double> &weight);
 
 struct cup2d_amr;
 // distributed contexts (cup2d_amr_create_ranks): refresh the halo slots of `field` from the owners (whole-block peer pulls,

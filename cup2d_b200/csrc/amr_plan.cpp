@@ -118,6 +118,9 @@ struct LabBuilder {
     if (which == 0) { dim = 2; sx = sy = -3; ex = ey = 4; tens = true; vector_bc = true; }
     else if (which == 1) { dim = 2; sx = sy = -1; ex = ey = 2; tens = false; vector_bc = true; }
     else if (which == 2) { dim = 1; sx = sy = -1; ex = ey = 2; tens = false; vector_bc = false; }
+    // 4, 5: the labs adapt() refines a block from (main.cpp:4908-4967): +-1 with corners, vector / scalar wall rules
+    else if (which == 4) { dim = 2; sx = sy = -1; ex = ey = 2; tens = true; vector_bc = true; }
+    else if (which == 5) { dim = 1; sx = sy = -1; ex = ey = 2; tens = true; vector_bc = false; }
     else { dim = 1; sx = sy = -4; ex = ey = 5; tens = true; vector_bc = false; } // GradChiOnTmp's chi lab (main.cpp:4633)
     nmx = BS + ex - sx - 1, nmy = BS + ey - sy - 1;
     ox = cdiv(sx - 1, 2) - 1, oy = cdiv(sy - 1, 2) - 1;
@@ -404,34 +407,58 @@ struct cup2d_amr_plan {
   std::vector<int32_t> irregular; // blocks with a coarser or finer block among their 8 neighbours
   GhostTable ghosts[4];
   // CSR per stencil kind: rows = (block, iy, ix, comp)
-  std::vector<int64_t> rowptr[4];
-  std::vector<int32_t> src_block[4], src_cc[4]; // source block, source cell*dim + comp
-  std::vector<double> w[4];
+  std::vector<int64_t> rowptr[6];
+  std::vector<int32_t> src_block[6], src_cc[6]; // source block, source cell*dim + comp
+  std::vector<double> w[6];
   // coarse-fine faces: (fine block, fine face, coarse block, coarse face, half)
   std::vector<int32_t> faces;
-  bool built[4] = {false, false, false, false};
+  bool built[6] = {false, false, false, false, false, false};
 };
 
-static void build(cup2d_amr_plan *p, int which) {
-  LabBuilder lb(p->mesh, which);
-  const int n = (int)p->mesh.lij.size() / 3;
-  auto &rp = p->rowptr[which];
+// full lab rows of the blocks `ks` (in that order) for stencil kind `which`, appended to the CSR (rp, sb, sc, w)
+static void lab_rows(const Mesh &mesh, int which, const int32_t *ks, int64_t n, std::vector<int64_t> &rp, std::vector<int32_t> &sb,
+                     std::vector<int32_t> &sc, std::vector<double> &w) {
+  LabBuilder lb(mesh, which);
   rp.assign(1, 0);
-  for (int k = 0; k < n; k++) {
-    lb.load(k);
+  for (int64_t q = 0; q < n; q++) {
+    lb.load(ks[q]);
     for (auto &row : lb.m) {
       if (row.set)
         for (auto &t : row.t) {
           if (t.second == 0.0) continue;
-          const int64_t cellcomp = t.first % (64 * lb.dim);
-          p->src_block[which].push_back((int32_t)(t.first / (64 * lb.dim)));
-          p->src_cc[which].push_back((int32_t)cellcomp);
-          p->w[which].push_back(t.second);
+          sb.push_back((int32_t)(t.first / (64 * lb.dim)));
+          sc.push_back((int32_t)(t.first % (64 * lb.dim)));
+          w.push_back(t.second);
         }
-      rp.push_back((int64_t)p->w[which].size());
+      rp.push_back((int64_t)w.size());
     }
   }
+}
+
+static void build(cup2d_amr_plan *p, int which) {
+  const int n = (int)p->mesh.lij.size() / 3;
+  std::vector<int32_t> all(n);
+  for (int k = 0; k < n; k++) all[k] = k;
+  lab_rows(p->mesh, which, all.data(), n, p->rowptr[which], p->src_block[which], p->src_cc[which], p->w[which]);
   p->built[which] = true;
+}
+
+const std::vector<int> &amr_plan_level_ij(const cup2d_amr_plan *p, int *bpdx, int *bpdy) {
+  *bpdx = p->mesh.bpdx, *bpdy = p->mesh.bpdy;
+  return p->mesh.lij;
+}
+
+// the full lab rows of a subset of blocks (csrc/amr_regrid.cu: the parents a regrid refines), without building or caching the
+// table of the whole mesh
+int amr_plan_subset_rows(cup2d_amr_plan *p, int which, int64_t nsub, const int32_t *blocks, std::vector<int64_t> &rowptr,
+                         std::vector<int32_t> &src_block, std::vector<int32_t> &src_cellcomp, std::vector<double> &weight) {
+  if (!p || which < 0 || which > 5 || nsub < 0) return CUP2D_EINVAL;
+  const int64_t n = (int64_t)p->mesh.lij.size() / 3;
+  for (int64_t q = 0; q < nsub; q++)
+    if (blocks[q] < 0 || blocks[q] >= n) return CUP2D_EINVAL;
+  src_block.clear(), src_cellcomp.clear(), weight.clear();
+  lab_rows(p->mesh, which, blocks, nsub, rowptr, src_block, src_cellcomp, weight);
+  return CUP2D_OK;
 }
 
 // ---- compact ghost tables -----------------------------------------------------------------------------------------
@@ -687,7 +714,7 @@ int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int6
 
 int64_t cup2d_amr_plan_stencil(cup2d_amr_plan *p, int which, int64_t *rowptr, int32_t *src_block, int32_t *src_cellcomp,
                                double *weight) {
-  if (!p || which < 0 || which > 3) return CUP2D_EINVAL;
+  if (!p || which < 0 || which > 5) return CUP2D_EINVAL;
   if (!p->built[which]) build(p, which);
   const int64_t nnz = (int64_t)p->w[which].size();
   if (rowptr) memcpy(rowptr, p->rowptr[which].data(), p->rowptr[which].size() * sizeof(int64_t));
@@ -849,6 +876,197 @@ int cup2d_amr_plan_neighbours(cup2d_amr_plan *p, int32_t *out) {
     }
   }
   return CUP2D_OK;
+}
+
+/* ---- adapt()'s refine / compress decision (main.cpp:4676-4860) and the order of the new block list (fill_pos, Encode:
+ * main.cpp:1550-1553, 422-445, SpaceCurve 342-421 and 6342-6376).  Host only: a pure function of the block list and the
+ * per-block L-inf of the tagging field (cup2d_amr_adapt_tags).  The states are updated in place in the reference's loop
+ * order (blocks in list order, levels from levelMax-1 down), so the result is the reference's, order effects included.
+ * Neighbour positions outside the domain are skipped; the reference wraps their index, which differs only on a level with a
+ * single block row or column. */
+namespace {
+struct Curve { // SpaceCurve::forward / inverse / Encode
+  int bpdx, bpdy, lmax, base = 0;
+  bool regular = true;
+  std::vector<int64_t> zsave;            // [j * bpdx + i]
+  std::vector<std::array<int, 2>> inv;   // zsave value -> (i, j)
+  static int64_t xy2d(int b, int x, int y) {
+    const int n = 1 << b;
+    int64_t d = 0;
+    for (int s = n / 2; s > 0; s /= 2) {
+      const int rx = (x & s) > 0, ry = (y & s) > 0;
+      d += (int64_t)s * s * ((3 * rx) ^ ry);
+      if (ry == 0) {
+        if (rx == 1) x = n - 1 - x, y = n - 1 - y;
+        std::swap(x, y);
+      }
+    }
+    return d;
+  }
+  static void d2xy(int b, int64_t t, int &x, int &y) {
+    const int n = 1 << b;
+    x = y = 0;
+    for (int64_t s = 1; s < n; s *= 2) {
+      const int64_t rx = 1 & (t / 2), ry = 1 & (t ^ rx);
+      if (ry == 0) {
+        if (rx == 1) x = (int)s - 1 - x, y = (int)s - 1 - y;
+        std::swap(x, y);
+      }
+      x += (int)(s * rx), y += (int)(s * ry);
+      t /= 4;
+    }
+  }
+  Curve(int bx, int by, int lm) : bpdx(bx), bpdy(by), lmax(lm), zsave((size_t)bx * by), inv((size_t)bx * by) {
+    while ((1 << base) < std::max(bx, by)) base++;
+    for (int j = 0; j < by; j++)
+      for (int i = 0; i < bx; i++) {
+        int64_t index = xy2d(base, i, j), sub = 0;
+        for (int64_t h = 0; h < index; h++) {
+          int x, y;
+          d2xy(base, h, x, y);
+          sub += x >= bx || y >= by;
+        }
+        if (sub) regular = false;
+        zsave[(size_t)j * bx + i] = index - sub;
+        inv[index - sub] = {i, j};
+      }
+  }
+  int64_t forward(int l, int i, int j) const {
+    if (l >= lmax) return 0;
+    if (regular) return xy2d(l + base, i, j);
+    const int aux = 1 << l, I = i / aux, J = j / aux;
+    return xy2d(l, i - I * aux, j - J * aux) + zsave[(size_t)J * bpdx + I] * aux * aux;
+  }
+  void inverse(int64_t Z, int l, int &i, int &j) const {
+    if (regular) return d2xy(l + base, Z, i, j);
+    const int64_t aux = 1LL << l;
+    d2xy(l, Z % (aux * aux), i, j);
+    const auto &IJ = inv[(size_t)(Z / (aux * aux))];
+    i += IJ[0] * (int)aux, j += IJ[1] * (int)aux;
+  }
+  int64_t encode(int level, int i, int j) const {
+    int64_t r = 0;
+    for (int l = level, ix = i, iy = j; l >= 0; l--, ix /= 2, iy /= 2) r += forward(l, ix, iy);
+    int ix = 2 * i, iy = 2 * j;
+    for (int l = level + 1; l < lmax; l++) {
+      int64_t Zc = forward(l, ix, iy);
+      Zc -= Zc % 4;
+      r += Zc;
+      int ix1, iy1;
+      inverse(Zc, l, ix1, iy1);
+      ix = 2 * ix1, iy = 2 * iy1;
+    }
+    return r + level;
+  }
+};
+enum { LEAVE = 0, REFINE = 1, COMPRESS = 2 };
+} // namespace
+
+int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, int32_t level_max,
+                             const double *block_linf, double rtol, double ctol, int32_t *new_level_ij) {
+  if (!level_ij || !block_linf || nblocks <= 0 || bpdx <= 0 || bpdy <= 0 || level_max < 1 || level_max > 20) {
+    cup2d::set_error("cup2d_amr_adapt_mesh: bad arguments");
+    return CUP2D_EINVAL;
+  }
+  Mesh m;
+  m.bpdx = bpdx, m.bpdy = bpdy;
+  m.lij.assign(level_ij, level_ij + 3 * nblocks);
+  for (int64_t k = 0; k < nblocks; k++) {
+    const int l = level_ij[3 * k], i = level_ij[3 * k + 1], j = level_ij[3 * k + 2];
+    if (l < 0 || l >= level_max || i < 0 || j < 0 || i >= (bpdx << l) || j >= (bpdy << l) || m.index.count({l, i, j})) {
+      cup2d::set_error("cup2d_amr_adapt_mesh: block " + std::to_string(k) + " is outside the domain, above levelMax-1 or duplicated");
+      return CUP2D_EINVAL;
+    }
+    m.index[{l, i, j}] = (int)k;
+  }
+  std::vector<int> st(nblocks);
+  auto state_at = [&](int l, int i, int j) { // state of an existing block, LEAVE for a position without one
+    const int k = m.find(l, i, j);
+    return k < 0 ? (int)LEAVE : st[k];
+  };
+  for (int64_t k = 0; k < nblocks; k++) { // main.cpp:4682-4688
+    const int l = level_ij[3 * k];
+    int s = block_linf[k] > rtol ? REFINE : block_linf[k] < ctol ? COMPRESS : LEAVE;
+    if ((s == REFINE && l == level_max - 1) || (s == COMPRESS && l == 0)) s = LEAVE;
+    st[k] = s;
+  }
+  auto neighbours = [&](int l, int I, int J, auto &&visit) { // in the reference's (x outer, y inner) order; false stops
+    const int NX = bpdx << l, NY = bpdy << l;
+    const bool xskin = I == 0 || I == NX - 1, yskin = J == 0 || J == NY - 1;
+    const int xskip = I == 0 ? -1 : 1, yskip = J == 0 ? -1 : 1;
+    for (int x = -1; x < 2; x++)
+      for (int y = -1; y < 2; y++) {
+        if ((x == 0 && y == 0) || (x == xskip && xskin) || (y == yskip && yskin)) continue;
+        if (I + x < 0 || I + x >= NX || J + y < 0 || J + y >= NY) continue;
+        if (!visit(x, y)) return;
+      }
+  };
+  for (int lv = level_max - 1; lv >= 0; lv--) {
+    for (int64_t k = 0; k < nblocks; k++) { // main.cpp:4735-4785: finer neighbours
+      const int l = level_ij[3 * k], I = level_ij[3 * k + 1], J = level_ij[3 * k + 2];
+      if (l != lv || st[k] == REFINE || l == level_max - 1) continue;
+      neighbours(l, I, J, [&](int x, int y) {
+        if (m.state(l, I + x, J + y) != -1) return true;
+        if (st[k] == COMPRESS) st[k] = LEAVE;
+        const int Bstep = abs(x) + abs(y) == 2 ? 3 : 1;
+        for (int B = 0; B <= 1; B += Bstep) {
+          const int aux = abs(x) == 1 ? B % 2 : B / 2;
+          const int iN = 2 * I + std::max(x, 0) + x + (B % 2) * std::max(0, 1 - abs(x));
+          const int jN = 2 * J + std::max(y, 0) + y + aux * std::max(0, 1 - abs(y));
+          if (state_at(lv + 1, iN, jN) == REFINE) {
+            st[k] = REFINE;
+            return false;
+          }
+        }
+        return true;
+      });
+    }
+    if (lv == 0) break;
+    for (int64_t k = 0; k < nblocks; k++) { // main.cpp:4791-4823: a same-level neighbour refines
+      const int l = level_ij[3 * k], I = level_ij[3 * k + 1], J = level_ij[3 * k + 2];
+      if (l != lv || st[k] != COMPRESS) continue;
+      neighbours(l, I, J, [&](int x, int y) {
+        if (state_at(l, I + x, J + y) != REFINE) return true;
+        st[k] = LEAVE;
+        return false;
+      });
+    }
+  }
+  for (int64_t k = 0; k < nblocks; k++) { // main.cpp:4825-4860: all four siblings compress, or none does
+    const int l = level_ij[3 * k], I = level_ij[3 * k + 1], J = level_ij[3 * k + 2];
+    const int i0 = 2 * (I / 2), j0 = 2 * (J / 2);
+    bool all = true;
+    for (int a = 0; a < 2; a++)
+      for (int b = 0; b < 2; b++) {
+        const int s = m.find(l, i0 + a, j0 + b);
+        all = all && s >= 0 && st[s] == COMPRESS;
+      }
+    if (all) continue;
+    for (int a = 0; a < 2; a++)
+      for (int b = 0; b < 2; b++) {
+        const int s = m.find(l, i0 + a, j0 + b);
+        if (s >= 0 && st[s] == COMPRESS) st[s] = LEAVE;
+      }
+  }
+  std::vector<std::array<int, 3>> out; // main.cpp:4926-5195, then fill_pos
+  for (int64_t k = 0; k < nblocks; k++) {
+    const int l = level_ij[3 * k], i = level_ij[3 * k + 1], j = level_ij[3 * k + 2];
+    if (st[k] == REFINE)
+      for (int b = 0; b < 2; b++)
+        for (int a = 0; a < 2; a++) out.push_back({l + 1, 2 * i + a, 2 * j + b});
+    else if (st[k] == COMPRESS) {
+      if (i % 2 == 0 && j % 2 == 0) out.push_back({l - 1, i / 2, j / 2});
+    } else
+      out.push_back({l, i, j});
+  }
+  if (new_level_ij) {
+    const Curve curve(bpdx, bpdy, level_max);
+    std::vector<std::pair<int64_t, size_t>> key(out.size());
+    for (size_t q = 0; q < out.size(); q++) key[q] = {curve.encode(out[q][0], out[q][1], out[q][2]), q};
+    std::sort(key.begin(), key.end());
+    for (size_t q = 0; q < out.size(); q++) memcpy(new_level_ij + 3 * q, out[key[q].second].data(), 3 * sizeof(int32_t));
+  }
+  return (int64_t)out.size();
 }
 
 int64_t cup2d_amr_plan_faces(cup2d_amr_plan *p, int32_t *out) {

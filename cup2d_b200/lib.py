@@ -30,6 +30,7 @@ SYMBOLS = [
     "cup2d_amr_penalize", "cup2d_amr_udef_assemble", "cup2d_amr_adapt_tags", "cup2d_amr_set_ranks", "cup2d_amr_peer_export",
     "cup2d_amr_peer_attach", "cup2d_peer_field_ptr", "cup2d_amr_dump", "cup2d_amr_create_ranks", "cup2d_amr_advect_diffuse_rhs_fast",
     "cup2d_amr_pressure_rhs_fast", "cup2d_amr_pressure_gradient_fast", "cup2d_amr_laplacian_fast", "cup2d_amr_set_fast",
+    "cup2d_amr_adapt_mesh", "cup2d_amr_regrid",
 ]
 
 
@@ -146,6 +147,10 @@ def load_library():
     lib.cup2d_amr_adapt_tags.argtypes = [P, D, I, C.POINTER(D)]
     lib.cup2d_amr_set_ranks.argtypes = [P, I, I, C.POINTER(C.c_int64)]
     lib.cup2d_amr_dump.argtypes = [P, D, C.c_char_p]
+    lib.cup2d_amr_adapt_mesh.argtypes = [L, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32, C.POINTER(D), D, D,
+                                         C.POINTER(C.c_int32)]
+    lib.cup2d_amr_adapt_mesh.restype = L
+    lib.cup2d_amr_regrid.argtypes = [P, L, C.POINTER(C.c_int32)]
     lib.cup2d_amr_create_ranks.argtypes = [L, C.POINTER(C.c_int32), I, I, D, D, I, I, C.POINTER(C.c_int64), I, C.POINTER(P)]
     lib.cup2d_amr_peer_export.argtypes = [P, P]
     lib.cup2d_amr_peer_attach.argtypes = [P, P]

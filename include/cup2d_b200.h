@@ -327,12 +327,25 @@ int cup2d_amr_peer_attach(cup2d_amr *a, const void *all_blobs);
  * k of the field adapt() thresholds against Rtol / Ctol — the vorticity of vel (KernelVorticity, 3343-3366), with 2*rtol in
  * the four centre cells of every block whose chi lab (stencil {-4,-4,5,5,tensorial}, ghosts across level jumps included) is
  * positive within 4 cells (finest level, level_max - 1) or 2 cells (other levels) of it (GradChiOnTmp, 4631-4656).  The
- * field itself is left in tmp.  States, 2:1 balancing and the mesh surgery stay on the host. */
+ * field itself is left in tmp.  The decision is cup2d_amr_adapt_mesh, the field transfer cup2d_amr_regrid. */
 int cup2d_amr_adapt_tags(cup2d_amr *a, double rtol, int level_max, double *block_linf_out);
 
 /* dump() on a multi-level mesh (main.cpp:3367-3467; cf. cup2d_dump): path.xdmf2, path.xyz.raw, path.attr.raw — the
  * reference's three files, byte for byte, from the device-resident velocity. */
 int cup2d_amr_dump(cup2d_amr *a, double time, const char *path);
+/* adapt()'s refine / compress decision, host only, no GPU needed (main.cpp:4676-4860: thresholds, Refine at levelMax-1 and
+ * Compress at level 0 dropped, the 2:1 pass from levelMax-1 down with the reference's in-place updates, sibling agreement),
+ * then the new block list in the reference's order (fill_pos / Encode, main.cpp:1550-1553, 422-445).  block_linf = the
+ * per-block L-inf of cup2d_amr_adapt_tags.  Returns the new block count; new_level_ij may be NULL to size it first. */
+int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, int32_t level_max,
+                             const double *block_linf, double rtol, double ctol, int32_t *new_level_ij);
+/* adapt()'s field transfer on the device (main.cpp:4902-5195; csrc/amr_regrid.cu): the context moves in place onto a mesh one
+ * refine / compress step away.  Copies unchanged blocks, refines from the {-1,-1,2,2,tensorial} lab of the old mesh
+ * (main.cpp:5012-5028), compresses by the reference's 4-cell average (5160-5164) for tmp, chi, vel, vold, pres, pold; tmpV is
+ * zero afterwards.  Plan, tables, Poisson context and lab buffers are rebuilt for the new mesh; shapes are cleared (set them
+ * again, as ongrid() does after adapt()).  CUP2D_EINVAL, context untouched, for a mesh that is not one step away;
+ * CUP2D_ESTATE for contexts on several ranks.  The same block list is a no-op. */
+int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level_ij);
 
 /* Bodies on a multi-level mesh: the cup2d_shape_* calls (above) on the cup2d_amr context, with the cell size and the block
  * position taken per block (Info::h, Info::origin, main.cpp:695-696).  block_ids index the context's blocks; a shape's

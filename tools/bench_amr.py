@@ -4,6 +4,7 @@ reference grows for its run.sh case (config C5 of SURVEY 8(d) at the chosen leve
   python tools/bench_amr.py [levelMax=9] [steps=10] [poisson_iters=10] [fast=1]
   python tools/bench_amr.py synthetic [base_level=9] [steps=10] [poisson_iters=10] [fast=1]     (config C5: 3 levels;
       under torchrun on N GPUs: the mesh distributed by block ranges, cup2d_amr_create_ranks)
+  python tools/bench_amr.py regrid [base_level=9]      one adapt() of the C5 mesh: decision, regrid, transfer kernels
 
 The mesh comes from oracle/_ref/ref_harness amrlab (which travels to the GPU box prebuilt), the fields are its seeded ones,
 bodies are left out (u_def = 0, chi = 0).  Prints one JSON line: blocks, cells, levels, ms per step with CUDA events on the
@@ -92,7 +93,67 @@ def run(sim, nb, blocks, steps, K, label, t_create, fast):
                       "Mcell_updates_per_s": cells * (2 + K) / wall / 1e6, "create_s": t_create}))
 
 
+def regrid(base):
+    """one adapt() of the C5 synthetic mesh with seeded fields, tolerances at quantiles of the device's tagging field so that a
+    sizeable share of the blocks refines and of the groups compresses: host time of the decision (cup2d_amr_adapt_mesh), wall
+    time of cup2d_amr_regrid, device time of its transfer kernels (torch.profiler), their bytes per new cell against the
+    algorithmic figure (each of the six transferred fields read once and written once: 2 x 8 doubles = 128 B per cell, plus
+    the lab gather of the refined parents)"""
+    import torch
+    from cup2d_b200.amr import AmrSimulation, adapt_mesh
+    blocks = three_level_mesh(base)
+    h0, lmax = 1.0 / 8, base + 4   # one level of headroom: the finest blocks may refine too
+    vel, pres = seeded_fields(blocks, h0)
+    rng = np.random.default_rng(0)
+    vel = vel + 0.05 * rng.uniform(-1, 1, vel.shape)
+    sim = AmrSimulation(blocks, 1, 1, h0, 1e-4)
+    for n, a in (("vel", vel), ("vold", vel), ("pres", pres), ("pold", pres), ("tmp", pres)):
+        sim.upload(n, a)
+    linf = sim.adapt_tags(1e300, lmax)
+    rtol, ctol = float(np.quantile(linf, 0.9)), float(np.quantile(linf, 0.4))
+    t0 = time.perf_counter()
+    new = adapt_mesh(blocks, 1, 1, lmax, linf, rtol, ctol)
+    t_decision = time.perf_counter() - t0
+    old = {tuple(b): k for k, b in enumerate(blocks.tolist())}
+    nref = sum((l - 1, i // 2, j // 2) in old for l, i, j in new.tolist()) // 4
+    ncomp = sum((l + 1, 2 * i, 2 * j) in old for l, i, j in new.tolist())
+    from cup2d_b200.amr import AmrPlan
+    t0 = time.perf_counter()
+    AmrPlan(new, 1, 1).close()
+    t_plan = time.perf_counter() - t0
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        t0 = time.perf_counter()
+        sim.regrid(new)
+        t_wall = time.perf_counter() - t0
+        torch.cuda.synchronize()
+    dev = {}
+    for e in prof.events():
+        if e.name.startswith("amr_regrid_") or "amr_regrid_" in e.name:
+            k = e.name.split("(")[0].split("::")[-1].replace("void ", "")
+            dev[k] = dev.get(k, 0.0) + getattr(e, "device_time_total", 0.0) * 1e-6
+    t_dev = sum(dev.values())
+    cells = len(new) * 64
+    algo = 128 * cells + nref * (100 * 2 * 2 + 100 * 4) * 8   # + the parents' labs (2 vector + 4 scalar fields), read and written
+    props = torch.cuda.get_device_properties(0)
+    try:
+        import subprocess as sp
+        power = sp.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    except Exception:
+        power = "unknown"
+    print(json.dumps({"workload": f"regrid of the synthetic 3-level mesh, base level {base}", "blocks_old": len(blocks),
+                      "blocks_new": len(new), "refined": nref, "compressed_groups": ncomp, "t_decision_s": t_decision,
+                      "t_new_plan_s": t_plan, "t_regrid_wall_s": t_wall, "t_host_part_s": t_wall - t_dev,
+                      "t_transfer_device_s": t_dev, "per_kernel_s": dev,
+                      "bytes_per_cell_algorithmic": algo / cells, "GB_per_s_algorithmic": algo / t_dev / 1e9 if t_dev else None,
+                      "gpu": props.name, "power_limit": power}))
+    sim.close()
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "regrid":      # python tools/bench_amr.py regrid [base_level=9]
+        regrid(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "synthetic":   # python tools/bench_amr.py synthetic [base_level=9] [steps] [K] [fast]
         base = int(sys.argv[2]) if len(sys.argv) > 2 else 9
         steps = int(sys.argv[3]) if len(sys.argv) > 3 else 10
