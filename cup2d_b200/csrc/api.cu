@@ -601,7 +601,7 @@ int64_t cup2d_launch_count(const cup2d_sim *s) { return s ? s->launches : 0; }
 
 static const char *kclass_name[KC_COUNT] = {"advect_stage_kernel", "umax_kernel", "pressure_rhs_kernel",
     "pressure_correct_kernel", "k_init", "k_pupdate", "k_spmv<0>", "k_r_update", "k_spmv<1>", "k_final",
-    "halo_pull_kernel", "vorticity_tag_kernel"};
+    "k_p_spmv", "k_r_spmv", "k_x_final", "halo_pull_kernel", "vorticity_tag_kernel"};
 int cup2d_profile_enable(cup2d_sim *s, int on) {
   if (!s) return CUP2D_EINVAL;
   s->prof.clear(); // the events stay in the pool and are reused
@@ -839,7 +839,7 @@ static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, d
   cudaGraph_t cap_graph = nullptr;
   if (capturing && tol && max_iter > 0) {
     // tolerance-driven solve inside a graph: a WHILE node whose body is one iteration.  Its condition starts at 1 on
-    // every launch; the last CTA of k_init and of every k_final sets it to !done (cudaGraphSetConditional).
+    // every launch; the last CTA of k_init and of every k_final / k_x_final sets it to !done (cudaGraphSetConditional).
     cudaStreamCaptureStatus st;
     CUP2D_CUDA(cudaStreamGetCaptureInfo(s->stream, &st, nullptr, &cap_graph, nullptr, nullptr));
     cudaGraphConditionalHandle handle;

@@ -14,12 +14,14 @@
 //     (set_alpha/beta/omega/rho, cuda.cu:303-330) run in the last CTA of the producing kernel, the
 //     x_opt snapshot (cuda.cu:537) is a rotation among three x buffers, and convergence is a device
 //     flag that turns the remaining launches into no-ops.
+// (On one rank with a uniform grid the five kernels become three, 136 B/cell: see k_p_spmv below.)
 // Traffic per iteration: 23 doubles/cell = 184 B/cell (SURVEY.md §8(d) budgets 25 = 200 B): the half-step update
 // x' = x + alpha z of cuda.cu:498 is deferred into the final kernel, which applies x'' = (x + alpha z_p) + omega z_r
 // in the reference's order (bitwise the same iterate), so the middle kernel neither reads nor writes x or z_p.
 // Memory access: warp-cooperative coalesced rows through padded shared memory (rows.cuh).
 #include "rows.cuh"
 #include "sim.h"
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <type_traits>
@@ -452,6 +454,261 @@ k_final(double *x0, double *x1, double *x2, const double *__restrict__ zp, const
   });
 }
 
+// ==== single-rank uniform grids: the same iteration in three kernels that recompute z = M p and z_r = M r ================
+// M is block-local (about 19 FP64 operations per cell), so recomputing it is cheaper than writing z and reading it back:
+// the iteration moves 17 doubles per cell instead of 23.  What stands in the way is the SpMV after each preconditioner: it
+// needs z on the face-neighbour blocks, and z there depends on the whole neighbour block.  So the two SpMV kernels work on
+// the advect stage's tiles (4x4 blocks + their 16 ring blocks) and precondition the ring blocks themselves:
+//   k_p_spmv  (KA): p' = r + beta (p - omega nu) ; z = M p' on tile + ring ; nu' = A z ; rhat.nu' -> alpha      r p nu rhat | p' nu'
+//   k_r_spmv  (KB): r' = r - alpha nu' ; z_r = M r' on tile + ring ; t = A z_r ; t.r', t.t -> omega               r nu'       | t
+//   k_x_final (KC): r' again ; z_p, z_r block-locally ; x = (x + alpha z_p) + omega z_r ; r = r' - omega t ; sums  x p' r nu' t rhat | x r
+// Every element-wise value is computed by the same expression as in the five-kernel path above; only the partition of the
+// dot products differs.  KA reads p and nu of ring blocks, so it must not write them in place: (p, nu) alternate between
+// (kp, knu) and (kz, kzr) by the parity of the iteration count (k_init zeroes the first pair), which one captured iteration
+// body of the graph WHILE node serves for every pass.
+#ifndef KTILE_CTAS
+#define KTILE_CTAS 2 // resident CTAs/SM the three kernels are register-bounded for (126-128 registers; at 3 (80) all of them spill)
+#endif
+constexpr int PST = 34; // tile plane row stride in doubles: 16-byte rows, conflict-free 128-bit row reads of a warp
+
+__device__ __forceinline__ int pair_in(const KrylovState *st) { return st->iter & 1; }
+
+// chunk layout of the warp's four blocks (any slots; -1 = absent): c[j] = piece `lane` of block sl[j] (as chunk_ld for four
+// consecutive blocks, so chunk_to_rows / rows_to_chunk apply unchanged)
+__device__ __forceinline__ void blocks_ld(const double *__restrict__ f, const int (&sl)[4], int lane, double2 (&c)[4]) {
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+    c[j] = sl[j] >= 0 ? reinterpret_cast<const double2 *>(f + (size_t)sl[j] * 64)[lane] : make_double2(0.0, 0.0);
+}
+__device__ __forceinline__ void blocks_st(double *__restrict__ f, const int (&sl)[4], int lane, const double2 (&c)[4]) {
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+    if (sl[j] >= 0) reinterpret_cast<double2 *>(f + (size_t)sl[j] * 64)[lane] = c[j];
+}
+
+// Shared memory of a tile: z of the 16 interior blocks (plane rows 1..32), row 7 of the S ring blocks (plane row 0),
+// row 0 of the N ring blocks (plane row 33), column 7 of the W and column 0 of the E ring blocks.
+struct __align__(16) TileSmem {
+  double plane[34 * PST];
+  double wcol[32], ecol[32];
+};
+
+// Warp w holds the blocks tiles[4w .. 4w+3] in row layout (lane = block lane>>3, row lane&7): warps 0-3 the interior block
+// rows, warps 4-7 the W, E, S, N ring blocks.  v: the vector to precondition; on return the interior warps hold
+// out = A M v of their rows in chunk layout (zero for absent blocks).  All threads call.  Walls: ghost = own cell.
+__device__ __forceinline__ void tile_precond_lap(double (&v)[8], TileSmem &ts, double *sw, int lane, int warp,
+                                                 const int *__restrict__ tslots, double2 (&out)[4]) {
+  precond_row(v, sw, lane);
+  const int bx = lane >> 3, y = lane & 7;
+  __syncthreads(); // the previous tile's stencil reads of the plane are done
+  if (warp < 4) {
+    double2 *p = reinterpret_cast<double2 *>(ts.plane + (warp * 8 + y + 1) * PST + bx * 8);
+#pragma unroll
+    for (int k = 0; k < 4; k++) p[k] = make_double2(v[2 * k], v[2 * k + 1]);
+  } else if (warp == 4) {
+    ts.wcol[bx * 8 + y] = v[7];
+  } else if (warp == 5) {
+    ts.ecol[bx * 8 + y] = v[0];
+  } else if ((warp == 6 && y == 7) || (warp == 7 && y == 0)) {
+    double2 *p = reinterpret_cast<double2 *>(ts.plane + (warp == 6 ? 0 : 33) * PST + bx * 8);
+#pragma unroll
+    for (int k = 0; k < 4; k++) p[k] = make_double2(v[2 * k], v[2 * k + 1]);
+  }
+  __syncthreads();
+  if (warp >= 4) return;
+  const int by = warp, R = by * 8 + y;
+  double o[8];
+  if (tslots[by * 4 + bx] < 0) {
+#pragma unroll
+    for (int i = 0; i < 8; i++) o[i] = 0.0;
+  } else {
+    const bool hN = y < 7 || tslots[by < 3 ? (by + 1) * 4 + bx : 28 + bx] >= 0;
+    const bool hS = y > 0 || tslots[by > 0 ? (by - 1) * 4 + bx : 24 + bx] >= 0;
+    const bool hW = tslots[bx > 0 ? by * 4 + bx - 1 : 16 + by] >= 0;
+    const bool hE = tslots[bx < 3 ? by * 4 + bx + 1 : 20 + by] >= 0;
+    const double *pl = ts.plane + (R + 1) * PST + bx * 8;
+    const double2 *pu = reinterpret_cast<const double2 *>(pl + PST), *pd = reinterpret_cast<const double2 *>(pl - PST);
+    const double gW = hW ? (bx > 0 ? pl[-1] : ts.wcol[R]) : v[0];
+    const double gE = hE ? (bx < 3 ? pl[8] : ts.ecol[R]) : v[7];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+      const int i = 2 * k;
+      const double2 u = hN ? pu[k] : make_double2(v[i], v[i + 1]), d = hS ? pd[k] : make_double2(v[i], v[i + 1]);
+      const double w0 = i > 0 ? v[i - 1] : gW, e1 = i + 1 < 7 ? v[i + 2] : gE;
+      o[i] = (((d.x + w0) + v[i + 1]) + u.x) - 4.0 * v[i]; // summation order S,W,E,N then -4C (rows_lap_coop)
+      o[i + 1] = (((d.y + v[i]) + e1) + u.y) - 4.0 * v[i + 1];
+    }
+  }
+  rows_to_chunk(sw, lane, o, out);
+}
+
+#define TILE_LOOP()                                                                               \
+  __shared__ __align__(16) double s_scr[WPB * SCR1];                                              \
+  __shared__ TileSmem s_tile;                                                                     \
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;                                     \
+  double *sw = s_scr + warp * SCR1;                                                               \
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x)
+
+// ---- KA: p' = r + beta (p - omega nu) ; nu' = A M p' ; rhat.nu' -> alpha   (cuda.cu:478-496) ----------------------------
+__global__ void __launch_bounds__(NT, KTILE_CTAS)
+k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, double *p1, double *nu0, double *nu1,
+         const int *__restrict__ tiles, int ntiles, KrylovState *st, double *partials, unsigned int *counter, Comm comm) {
+  if (st->done) return;
+  const double beta = st->beta, nomega = -st->omega;
+  const bool restart = st->restart_now != 0;
+  const int in = pair_in(st);
+  const double *__restrict__ p = in ? p1 : p0;
+  const double *__restrict__ nu = in ? nu1 : nu0;
+  double *__restrict__ pn = in ? p0 : p1;
+  double *__restrict__ nun = in ? nu0 : nu1;
+  double sums[2] = {0, 0};
+  TILE_LOOP() {
+    const int *ts = tiles + (size_t)tile * TILE_SLOTS;
+    int sl[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) sl[j] = ts[4 * warp + j];
+    double2 cp[4], cr[4], ch[4];
+    blocks_ld(r, sl, lane, cr);
+    if (restart) {
+#pragma unroll
+      for (int j = 0; j < 4; j++) cp[j] = ch[j] = cr[j];
+      if (warp < 4) blocks_st(rhat, sl, lane, cr);
+    } else {
+      double2 cn[4];
+      blocks_ld(p, sl, lane, cp);
+      blocks_ld(nu, sl, lane, cn);
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        cp[j].x = fma(beta, fma(nomega, cn[j].x, cp[j].x), cr[j].x);
+        cp[j].y = fma(beta, fma(nomega, cn[j].y, cp[j].y), cr[j].y);
+      }
+    }
+    if (warp < 4) blocks_st(pn, sl, lane, cp);
+    double v[8];
+    chunk_to_rows(sw, lane, cp, v);
+    double2 ca[4];
+    tile_precond_lap(v, s_tile, sw, lane, warp, ts, ca);
+    if (warp < 4) {
+      if (!restart) blocks_ld(rhat, sl, lane, ch); // loaded late: held across the preconditioner it costs spills
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        sums[0] = fma(ca[j].x, ch[j].x, sums[0]);
+        sums[0] = fma(ca[j].y, ch[j].y, sums[0]);
+      }
+      blocks_st(nun, sl, lane, ca);
+    }
+  }
+  grid_reduce<2, NT>(sums, 0.0, partials, counter, comm, [=](const double *t, double) {
+    st->rhat_nu = t[0];
+    st->alpha = st->rho_curr / (t[0] + EPS21); // set_alpha
+    st->restart_now = 0;
+  });
+}
+
+// ---- KB: r' = r - alpha nu' ; t = A M r' ; t.r', t.t -> omega   (cuda.cu:499-518) -------------------------------------
+__global__ void __launch_bounds__(NT, KTILE_CTAS)
+k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, double *__restrict__ t,
+         const int *__restrict__ tiles, int ntiles, KrylovState *st, double *partials, unsigned int *counter, Comm comm) {
+  if (st->done) return;
+  const double alpha = st->alpha;
+  const double *__restrict__ nu = pair_in(st) ? nu0 : nu1; // what k_p_spmv of this iteration wrote
+  double sums[2] = {0, 0};
+  TILE_LOOP() {
+    const int *ts = tiles + (size_t)tile * TILE_SLOTS;
+    int sl[4];
+#pragma unroll
+    for (int j = 0; j < 4; j++) sl[j] = ts[4 * warp + j];
+    double2 cr[4], cn[4];
+    blocks_ld(r, sl, lane, cr);
+    blocks_ld(nu, sl, lane, cn);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      cr[j].x = fma(-alpha, cn[j].x, cr[j].x);
+      cr[j].y = fma(-alpha, cn[j].y, cr[j].y);
+    }
+    double v[8];
+    chunk_to_rows(sw, lane, cr, v);
+    double2 ca[4];
+    tile_precond_lap(v, s_tile, sw, lane, warp, ts, ca);
+    if (warp < 4) {
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        sums[0] = fma(ca[j].x, cr[j].x, sums[0]);
+        sums[0] = fma(ca[j].y, cr[j].y, sums[0]);
+        sums[1] = fma(ca[j].x, ca[j].x, sums[1]);
+        sums[1] = fma(ca[j].y, ca[j].y, sums[1]);
+      }
+      blocks_st(t, sl, lane, ca);
+    }
+  }
+  grid_reduce<2, NT>(sums, 0.0, partials, counter, comm, [=](const double *tsum, double) {
+    st->tr = tsum[0];
+    st->tt = tsum[1];
+    st->omega = tsum[0] / (tsum[1] + EPS21); // set_omega
+  });
+}
+
+// ---- KC: r' = r - alpha nu' ; x = (x + alpha M p') + omega M r' ; r = r' - omega t ; rhat.r, |r|^2, sum x, |r|_inf ----------
+// Block-local, so it keeps the chunk loop of k_final.  It writes r in place: every ring reader of r (k_r_spmv) has finished.
+__global__ void __launch_bounds__(NT, KTILE_CTAS)
+k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1, const double *nu0, const double *nu1,
+          double *__restrict__ r, const double *__restrict__ t, const double *__restrict__ rhat, int nrows,
+          KrylovState *st, double *partials, unsigned int *counter, Comm comm, unsigned long long loop_handle) {
+  __shared__ __align__(16) double s_scr[WPB * SCR1];
+  if (st->done) return;
+  const double alpha = st->alpha, omega = st->omega;
+  const int cur = st->cur, nxt = next_buf(st->cur, st->opt);
+  const double *xc = cur == 0 ? x0 : (cur == 1 ? x1 : x2);
+  double *xn = nxt == 0 ? x0 : (nxt == 1 ? x1 : x2);
+  const bool in = pair_in(st);
+  const double *__restrict__ p = in ? p0 : p1;
+  const double *__restrict__ nu = in ? nu0 : nu1;
+  double sums[3] = {0, 0, 0}; // rhat.r, r.r, sum x
+  double mx = 0;
+  CHUNK_LOOP() {
+    const int nv = min(32, nrows - row0);
+    double2 cz[4], cy[4], cr[4], cn[4];
+    double v[8];
+    chunk_ld(p, row0, nv, lane, cz);
+    chunk_ld(r, row0, nv, lane, cr);
+    chunk_ld(nu, row0, nv, lane, cn);
+    chunk_to_rows(sw, lane, cz, v);
+    precond_row(v, sw, lane);
+    rows_to_chunk(sw, lane, v, cz); // z_p
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      cr[j].x = fma(-alpha, cn[j].x, cr[j].x);
+      cr[j].y = fma(-alpha, cn[j].y, cr[j].y);
+    }
+    chunk_to_rows(sw, lane, cr, v);
+    precond_row(v, sw, lane);
+    rows_to_chunk(sw, lane, v, cy); // z_r
+    double2 cx[4], ct[4], ch[4];
+    chunk_ld(xc, row0, nv, lane, cx);
+    chunk_ld(t, row0, nv, lane, ct);
+    chunk_ld(rhat, row0, nv, lane, ch);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      cx[j].x = fma(omega, cy[j].x, fma(alpha, cz[j].x, cx[j].x)); // cuda.cu:498 then 520
+      cx[j].y = fma(omega, cy[j].y, fma(alpha, cz[j].y, cx[j].y));
+      cr[j].x = fma(-omega, ct[j].x, cr[j].x); // cuda.cu:524
+      cr[j].y = fma(-omega, ct[j].y, cr[j].y);
+      sums[0] = fma(ch[j].x, cr[j].x, sums[0]);
+      sums[0] = fma(ch[j].y, cr[j].y, sums[0]);
+      sums[1] = fma(cr[j].x, cr[j].x, sums[1]);
+      sums[1] = fma(cr[j].y, cr[j].y, sums[1]);
+      sums[2] += cx[j].x + cx[j].y;
+      mx = fmax(mx, fmax(fabs(cr[j].x), fabs(cr[j].y)));
+    }
+    chunk_st(xn, row0, nv, lane, cx);
+    chunk_st(r, row0, nv, lane, cr);
+  }
+  grid_reduce<3, NT>(sums, mx, partials, counter, comm, [=](const double *tsum, double m) {
+    end_of_iteration(st, tsum, m, nxt);
+    set_loop_condition(loop_handle, st);
+  });
+}
+
 static inline int red_grid(const cup2d_sim *s, int nrows) {
   int g = (nrows + NT - 1) / NT;
   int cap = s->num_sms * 8;
@@ -495,13 +752,39 @@ int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts
   return CUP2D_OK;
 }
 
-// n BiCGSTAB iterations: 5 kernels each, no host involvement (a converged solve turns them into no-ops)
+// n BiCGSTAB iterations, no host involvement (a converged solve turns them into no-ops): 3 kernels each on a single-rank
+// uniform grid; 5 with several ranks, general rows or no tiles (Poisson-only contexts)
 int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream) {
   const int nrows = (int)s->nloc * 8;
   const int grid = red_grid(s, nrows);
   const int4 *nbr = reinterpret_cast<const int4 *>(s->d_nbr);
   const bool has_irr = s->n_irr_rows > 0;
   const bool multi = s->nranks > 1;
+  if (!multi && !has_irr && !s->poisson_only) {
+    // one wave of tile CTAs: the tiles in flight then form one compact region of the Hilbert order, whose ring blocks
+    // are mostly read from L2
+    const int tgrid = std::min(grid, s->num_sms * KTILE_CTAS);
+    for (int k = 0; k < n; k++) {
+      {
+        ProfScope prof(s, KC_P_SPMV);
+        k_p_spmv<<<tgrid, NT, 0, stream>>>(s->kr, s->krhat, s->kp, s->kz, s->knu, s->kzr, s->d_tiles, s->ntiles, s->d_state,
+                                           s->d_partials, s->d_counter, s->comm);
+      }
+      {
+        ProfScope prof(s, KC_R_SPMV);
+        k_r_spmv<<<tgrid, NT, 0, stream>>>(s->kr, s->knu, s->kzr, s->kt, s->d_tiles, s->ntiles, s->d_state, s->d_partials,
+                                           s->d_counter, s->comm);
+      }
+      {
+        ProfScope prof(s, KC_X_FINAL);
+        k_x_final<<<grid, NT, 0, stream>>>(s->kx[0], s->kx[1], s->kx[2], s->kp, s->kz, s->knu, s->kzr, s->kr, s->kt, s->krhat,
+                                           nrows, s->d_state, s->d_partials, s->d_counter, s->comm, s->cond_handle);
+      }
+      s->launches += 3;
+    }
+    CUP2D_CUDA(cudaGetLastError());
+    return CUP2D_OK;
+  }
   const PushView pz = make_push(s, CUP2D_NFIELDS), pzr = make_push(s, CUP2D_NFIELDS + 4);
   const IrrView irr = irr_view(s);
   for (int k = 0; k < n; k++) {

@@ -146,7 +146,7 @@ struct cup2d_sim {
 
 namespace cup2d {
 enum KClass { KC_ADVECT = 0, KC_UMAX, KC_RHS, KC_CORRECT, KC_KINIT, KC_PUPDATE, KC_SPMV_NU, KC_XRUPDATE,
-              KC_SPMV_T, KC_FINAL, KC_HALO, KC_VORT, KC_COUNT };
+              KC_SPMV_T, KC_FINAL, KC_P_SPMV, KC_R_SPMV, KC_X_FINAL, KC_HALO, KC_VORT, KC_COUNT };
 // bracket one launch with events when profiling is on (no-op otherwise)
 struct ProfScope {
   cup2d_sim *s;
