@@ -270,6 +270,57 @@ class AmrSimulation:
     def udef_assemble(self):
         _l.check(self.lib.cup2d_amr_udef_assemble(self._h))
 
+    # ---- ongrid() on the device (cup2d_amr_ongrid) ----
+    MIDLINE = ("rX", "rY", "norX", "norY", "vX", "vY", "vNorX", "vNorY", "width")
+
+    def ongrid(self, bodies):
+        """ongrid()'s rasterisation (main.cpp:4019-4024, 4208-4556) of `bodies` into chi, tmp and the shapes' obstacle blocks.
+        A body is a mapping with the nine midline arrays of MIDLINE (shape frame, as at main.cpp:4208), "center", "orientation"
+        and "center_of_mass".  Returns [nshapes, 10]: Mass, COM_x, COM_y, new centre of mass x, y, m, j, u, v, a."""
+        arrs, structs = [], (_l.Body * len(bodies))()
+        for k, b in enumerate(bodies):
+            st = structs[k]
+            cols = [np.ascontiguousarray(b[n], dtype=np.float64) for n in self.MIDLINE]
+            nm = len(cols[0])
+            assert all(len(c) == nm for c in cols)
+            arrs.append(cols)
+            st.nm = nm
+            for n, c in zip(self.MIDLINE, cols):
+                setattr(st, n, c.ctypes.data_as(C.POINTER(C.c_double)))
+            st.center[0], st.center[1] = (float(x) for x in b["center"])
+            st.orientation = float(b["orientation"])
+            st.center_of_mass[0], st.center_of_mass[1] = (float(x) for x in b["center_of_mass"])
+        out = np.empty((len(bodies), 10))
+        _l.check(self.lib.cup2d_amr_ongrid(self._h, len(bodies), structs, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
+
+    ONGRID_TIMES = ("call", "scan", "offsets", "compact", "fish", "chi", "moments", "correct")
+
+    def ongrid_timing(self, on=True):
+        """time every following ongrid call with CUDA events on the context's stream (cup2d_amr_ongrid_timing)"""
+        _l.check(self.lib.cup2d_amr_ongrid_timing(self._h, int(on)))
+
+    def ongrid_times(self):
+        """milliseconds of the last timed ongrid call: dict over ONGRID_TIMES (the whole call, then each kernel class)"""
+        ms = np.empty(8)
+        _l.check(self.lib.cup2d_amr_ongrid_times(self._h, ms.ctypes.data_as(C.POINTER(C.c_double))))
+        return dict(zip(self.ONGRID_TIMES, ms.tolist()))
+
+    def shape_get(self, shape, dist=True):
+        """shape `shape`'s obstacle blocks on the device: dict of ids [nob], chi [nob,8,8], dist [nob,8,8] (shapes placed by
+        ongrid; None with dist=False) and udef [nob,8,8,2]"""
+        n = self.lib.cup2d_amr_shape_get(self._h, shape, None, None, None, None)
+        if n < 0:
+            _l.check(int(n))
+        ids, X, U = np.empty(n, dtype=np.int32), np.empty((n, 8, 8)), np.empty((n, 8, 8, 2))
+        Dd = np.empty((n, 8, 8)) if dist else None
+        P = C.POINTER(C.c_double)
+        rc = self.lib.cup2d_amr_shape_get(self._h, shape, ids.ctypes.data_as(C.POINTER(C.c_int32)), X.ctypes.data_as(P),
+                                          Dd.ctypes.data_as(P) if dist else None, U.ctypes.data_as(P))
+        if rc < 0:
+            _l.check(rc)
+        return {"ids": ids, "chi": X, "dist": Dd, "udef": U}
+
     def close(self):
         if self._h:
             self.lib.cup2d_amr_destroy(self._h)

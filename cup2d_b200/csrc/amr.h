@@ -59,6 +59,10 @@ int amr_plan_subset_rows(cup2d_amr_plan *p, int which, int64_t nsub, const int32
                          std::vector<int32_t> &src_block, std::vector<int32_t> &src_cellcomp, std::vector<double> &weight);
 
 struct cup2d_amr;
+// single-rank contexts: the fast path's neighbour / irregular-block / compact ghost tables (csrc/amr_fast.cu), built on first use
+int amr_fast_tables(cup2d_amr *a);
+// the per-block (i, j) table on the device, built on first use (csrc/amr_penalize.cu)
+int amr_ensure_ij(cup2d_amr *a);
 // distributed contexts (cup2d_amr_create_ranks): refresh the halo slots of `field` from the owners (whole-block peer pulls,
 // csrc/halo.cu) before a kernel reads neighbours; a no-op otherwise
 extern "C" int amr_dist_refresh(cup2d_amr *a, int field);
@@ -98,20 +102,35 @@ struct cup2d_amr {
   cup2d::GhostDev gt[3];            // compact ghost tables per stencil kind (cup2d_amr_plan_ghosts)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)
   // bodies (csrc/amr_penalize.cu): per-shape obstacle blocks, as cup2d_sim::Shape
-  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr; };
+  // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid: csrc/amr_ongrid.cu)
+  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false; };
   std::vector<Shape> shapes;
   std::vector<int32_t> h_ij;        // [nb][2] block index (i, j) at the block's own level (filled by cup2d_amr_create)
   int *d_ij = nullptr;              // the same on the device (first use)
   double *d_shape_part = nullptr;   // [cap][7] per-obstacle-block partial sums
   int shape_part_cap = 0;
   std::vector<double> h_shape_part;
+  // cup2d_amr_ongrid scratch (csrc/amr_ongrid.cu): staged midlines + segments, block masks, counts / offsets, per-block partials
+  double *d_og_stage = nullptr, *d_og_part = nullptr;
+  unsigned long long *d_og_mask = nullptr;
+  int *d_og_cnt = nullptr;
+  size_t og_stage_cap = 0, og_part_cap = 0, og_mask_cap = 0, og_cnt_cap = 0;
+  bool og_timing = false, og_timed = false; // cup2d_amr_ongrid_timing: CUDA events (cudaEvent_t) around the kernels of the last call
+  void *og_ev[12] = {};
+  void (*og_release)(cup2d_amr *) = nullptr; // destroys og_ev (set with them, csrc/amr_ongrid.cu)
   void free_shapes() {
     for (auto &sh : shapes) {
-      cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef);
+      cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);
     }
     shapes.clear();
     cudaFree(d_ij); cudaFree(d_shape_part);
     d_ij = nullptr, d_shape_part = nullptr, shape_part_cap = 0;
+    cudaFree(d_og_stage); cudaFree(d_og_part); cudaFree(d_og_mask); cudaFree(d_og_cnt);
+    d_og_stage = d_og_part = nullptr, d_og_mask = nullptr, d_og_cnt = nullptr;
+    og_stage_cap = og_part_cap = og_mask_cap = og_cnt_cap = 0;
+    if (og_release) og_release(this);
+    og_release = nullptr;
+    og_timing = og_timed = false;
   }
 };
 

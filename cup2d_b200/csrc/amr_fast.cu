@@ -364,6 +364,8 @@ static int fast_setup(cup2d_amr *a) {
 
 } // namespace cup2d
 
+int amr_fast_tables(cup2d_amr *a) { return cup2d::fast_setup(a); }
+
 // Tables of a DISTRIBUTED context: the plan knows the whole mesh; this rank keeps what concerns its blocks [b0, b1) and
 // names every block by its local slot (own blocks first, then the halo slots of the field arrays): slot_of[global block] or -1.
 int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64_t b0, int64_t b1) {

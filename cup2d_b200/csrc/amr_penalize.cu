@@ -145,6 +145,8 @@ static int ensure_ij(cup2d_amr *a) {
 
 } // namespace cup2d
 
+int amr_ensure_ij(cup2d_amr *a) { return cup2d::ensure_ij(a); }
+
 using namespace cup2d;
 
 #define CHECK_AMR_SHAPE(a, shape, must_exist)                                                     \
@@ -162,9 +164,10 @@ int cup2d_amr_shape_set(cup2d_amr *a, int shape, int nob, const int32_t *block_i
   CUP2D_CUDA(cudaSetDevice(a->device));
   if ((int)a->shapes.size() <= shape) a->shapes.resize(shape + 1);
   cup2d_amr::Shape &sh = a->shapes[shape];
+  sh.has_dist = false;
   if (nob > sh.cap) {
-    cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef);
-    sh.d_ids = nullptr; sh.d_X = sh.d_udef = nullptr;
+    cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);
+    sh.d_ids = nullptr; sh.d_X = sh.d_udef = sh.d_dist = nullptr;
     sh.cap = 0;
     const int cap = nob + nob / 4 + 16;
     CUP2D_CUDA(cudaMalloc(&sh.d_ids, (size_t)cap * sizeof(int)));

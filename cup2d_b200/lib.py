@@ -30,7 +30,8 @@ SYMBOLS = [
     "cup2d_amr_penalize", "cup2d_amr_udef_assemble", "cup2d_amr_adapt_tags", "cup2d_amr_set_ranks", "cup2d_amr_peer_export",
     "cup2d_amr_peer_attach", "cup2d_peer_field_ptr", "cup2d_amr_dump", "cup2d_amr_create_ranks", "cup2d_amr_advect_diffuse_rhs_fast",
     "cup2d_amr_pressure_rhs_fast", "cup2d_amr_pressure_gradient_fast", "cup2d_amr_laplacian_fast", "cup2d_amr_set_fast",
-    "cup2d_amr_adapt_mesh", "cup2d_amr_regrid",
+    "cup2d_amr_adapt_mesh", "cup2d_amr_regrid", "cup2d_amr_ongrid", "cup2d_amr_shape_get",
+    "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times",
 ]
 
 
@@ -45,6 +46,13 @@ class Config(C.Structure):
         ("rank_begin", C.POINTER(C.c_int64)), ("h", C.c_double), ("nu", C.c_double),
         ("cfl", C.c_double), ("device", C.c_int32), ("reserved", C.c_int32),
     ]
+
+
+class Body(C.Structure):
+    """cup2d_body: one shape's midline as ongrid() holds it at main.cpp:4208 (cup2d_amr_ongrid)"""
+    _fields_ = [("nm", C.c_int32), ("reserved", C.c_int32)] + [
+        (n, C.POINTER(C.c_double)) for n in ("rX", "rY", "norX", "norY", "vX", "vY", "vNorX", "vNorY", "width")] + [
+        ("center", C.c_double * 2), ("orientation", C.c_double), ("center_of_mass", C.c_double * 2)]
 
 
 _lib = None
@@ -151,6 +159,10 @@ def load_library():
                                          C.POINTER(C.c_int32)]
     lib.cup2d_amr_adapt_mesh.restype = L
     lib.cup2d_amr_regrid.argtypes = [P, L, C.POINTER(C.c_int32)]
+    lib.cup2d_amr_ongrid.argtypes = [P, I, C.POINTER(Body), C.POINTER(D)]
+    lib.cup2d_amr_ongrid_timing.argtypes = [P, I]
+    lib.cup2d_amr_ongrid_times.argtypes = [P, C.POINTER(D)]
+    lib.cup2d_amr_shape_get.argtypes = [P, I, C.POINTER(C.c_int32), C.POINTER(D), C.POINTER(D), C.POINTER(D)]
     lib.cup2d_amr_create_ranks.argtypes = [L, C.POINTER(C.c_int32), I, I, D, D, I, I, C.POINTER(C.c_int64), I, C.POINTER(P)]
     lib.cup2d_amr_peer_export.argtypes = [P, P]
     lib.cup2d_amr_peer_attach.argtypes = [P, P]

@@ -357,6 +357,36 @@ int cup2d_amr_penalize(cup2d_amr *a, int shape, double lambda, double dt, double
                        double omega);
 int cup2d_amr_udef_assemble(cup2d_amr *a);
 
+/* ongrid() on a multi-level mesh (main.cpp:3991-4630; csrc/amr_ongrid.cu): the rasterisation of every body's midline into the
+ * chi and tmp fields and into the shape's obstacle blocks, on the device.  The midline kinematics (main.cpp:4029-4207), the
+ * 3x3 rigid-body solve, the collision model and ComputeSurfaceNormals stay with the caller. */
+typedef struct {
+  int32_t nm, reserved;                /* midline points; nm >= 9 (Nsegments = (nm-1)/8 >= 1 dividing nm-1, main.cpp:4208-4210) */
+  const double *rX, *rY, *norX, *norY; /* [nm] each: the shape-frame midline exactly as ongrid() holds it at main.cpp:4208 */
+  const double *vX, *vY, *vNorX, *vNorY, *width;
+  double center[2], orientation;       /* Shape::center, Shape::orientation (already advanced by main.cpp:3993-4007) */
+  double center_of_mass[2];            /* Shape::centerOfMass before main.cpp:4485-4486 */
+} cup2d_body;
+/* main.cpp:4019-4024 + 4208-4556 for all shapes, in shape order: chi = 0 and tmp = -1 everywhere; the AreaSegment boxes
+ * (3839-3878, 4216-4242; safe distance 4 h with h the smallest cell of the mesh) on the host, with the host libm's cos / sin;
+ * the block scan (4243-4269), PutFishOnBlocks (4271-4463), PutChiOnGrid (3911-3969, 4469) and the rigid-motion removal
+ * (4472-4556) on the device.  out[10*k..] = {Mass, COM_x, COM_y (4475-4483), new centerOfMass x, y (4485-4486), m, j, u, v, a
+ * (4529-4531)}.  Leaves chi, tmp and each shape's obstacle blocks (ids in ascending block order, chi, dist, udef) on the device
+ * for cup2d_amr_shape_integrals / _penalize / _udef_assemble; shapes k >= nshapes are dropped.  dist, tmp and u_def before the
+ * correction are bit-identical to the reference; chi on blocks whose +-1 lab needs the ghost tables, and the sums, to rounding.
+ * CUP2D_EINVAL (context untouched) for a body with nm < 9 or (nm-1) not a multiple of (nm-1)/8, a missing array or its center outside the domain (the reference
+ * aborts, 4009-4013); CUP2D_ESTATE for contexts on several ranks.  1 <= nshapes <= 64. */
+int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double *out);
+/* download shape k's obstacle blocks (any pointer may be NULL; returns nob): ids[nob], chi[nob][64], dist[nob][64] (shapes placed
+ * by cup2d_amr_ongrid only), udef[nob][64][2] — what the host's collision model, forces and skins read */
+int cup2d_amr_shape_get(cup2d_amr *a, int shape, int32_t *ids, double *chi, double *dist, double *udef);
+/* CUDA-event timing of cup2d_amr_ongrid on the context's stream: timing(a, 1) creates the events and times every following call
+ * (0 stops; a regrid clears it); times(a, ms8) gives the last timed call's milliseconds: {whole call on the stream (upload,
+ * kernels and the host waits between them), scan, offsets, compact, fish, chi, moments, correct}, every kernel class summed
+ * over the shapes */
+int cup2d_amr_ongrid_timing(cup2d_amr *a, int on);
+int cup2d_amr_ongrid_times(cup2d_amr *a, double *ms8);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,6 +5,7 @@ reference grows for its run.sh case (config C5 of SURVEY 8(d) at the chosen leve
   python tools/bench_amr.py synthetic [base_level=9] [steps=10] [poisson_iters=10] [fast=1]     (config C5: 3 levels;
       under torchrun on N GPUs: the mesh distributed by block ranges, cup2d_amr_create_ranks)
   python tools/bench_amr.py regrid [base_level=9]      one adapt() of the C5 mesh: decision, regrid, transfer kernels
+  python tools/bench_amr.py ongrid [base_level=9]      cup2d_amr_ongrid of two fish in the finest region of the C5 mesh
 
 The mesh comes from oracle/_ref/ref_harness amrlab (which travels to the GPU box prebuilt), the fields are its seeded ones,
 bodies are left out (u_def = 0, chi = 0).  Prints one JSON line: blocks, cells, levels, ms per step with CUDA events on the
@@ -150,7 +151,62 @@ def regrid(base):
     sim.close()
 
 
+def ongrid(base, reps=20):
+    """cup2d_amr_ongrid of two run.sh-sized fish (L = 0.2 at the C5 scale: 0.2 / 4 of the unit square, Nm of the reference at
+    that resolution) inside the finest region of the C5 mesh, after warm-up: the whole call and each kernel class timed with CUDA
+    events on the context's stream (cup2d_amr_ongrid_timing; median over the calls), the host wall time per call, the
+    reset/scan kernel against its algorithmic bytes (16 B per cell + the block tables it reads: (i, j), h, the mask it writes),
+    and the PCIe bytes per step the call replaces (chi field upload 8 B/cell + the obstacle blocks)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import amr_body_oracle as bo
+    from cup2d_b200.amr import AmrSimulation
+    blocks = three_level_mesh(base)
+    h0 = 1.0 / 8
+    hmin = h0 / (1 << int(blocks[:, 0].max()))
+    L = 0.05
+    nm = 8 * int(np.ceil(L / (hmin / np.sqrt(2)) / 8)) + 1   # about the reference's midline spacing, minH / sqrt(2)
+    bodies = [bo.synthetic_body((0.48, 0.52), L, nm, 0.2), bo.synthetic_body((0.53, 0.50), L, nm, 3.0, phase=1.0)]
+    sim = AmrSimulation(blocks, 1, 1, h0, 1e-4)
+    for _ in range(3):
+        out = sim.ongrid(bodies)
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        sim.ongrid(bodies)          # returns after its last stream synchronisation
+    t_wall = (time.perf_counter() - t0) / reps
+    sim.ongrid_timing(True)
+    times = []
+    for _ in range(reps):
+        sim.ongrid(bodies)
+        times.append(sim.ongrid_times())
+    sim.ongrid_timing(False)
+    ms = {k: float(np.median([t[k] for t in times])) for k in sim.ONGRID_TIMES}
+    nb = len(blocks)
+    nob = [len(sim.shape_get(k, dist=False)["ids"]) for k in range(2)]
+    scan_bytes = nb * (64 * 16 + 8 + 8 + 8)
+    scan_s = ms["scan"] * 1e-3
+    import torch
+    props = torch.cuda.get_device_properties(0)
+    try:
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                               text=True).stdout.strip()
+    except Exception:
+        power = "unknown"
+    print(json.dumps({"workload": f"ongrid of two fish (Nm {nm}) on the synthetic 3-level mesh, base level {base}", "blocks": nb,
+                      "obstacle_blocks": nob, "t_call_events_ms": ms["call"], "t_call_wall_ms": t_wall * 1e3,
+                      "per_kernel_events_ms": {k: v for k, v in ms.items() if k != "call"},
+                      "t_kernels_ms": sum(v for k, v in ms.items() if k != "call"),
+                      "scan_bytes_algorithmic": scan_bytes, "scan_GB_per_s": scan_bytes / scan_s / 1e9 if scan_s else None,
+                      "pcie_bytes_removed_per_step": nb * 64 * 8 + sum(nob) * (4 + 64 * 8 + 128 * 8),
+                      "host_ongrid_time": "not measured at this size", "out": out.tolist(),
+                      "gpu": props.name, "power_limit": power}))
+    sim.close()
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "ongrid":      # python tools/bench_amr.py ongrid [base_level=9]
+        ongrid(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "regrid":      # python tools/bench_amr.py regrid [base_level=9]
         regrid(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
         return
