@@ -321,6 +321,27 @@ class AmrSimulation:
             _l.check(rc)
         return {"ids": ids, "chi": X, "dist": Dd, "udef": U}
 
+    # ---- the collision model on the device (cup2d_amr_collide) ----
+    def shape_set_dist(self, shape, dist):
+        """upload the signed distance [nob,8,8] of a shape set by shape_set (cup2d_amr_shape_set_dist)"""
+        dist = np.ascontiguousarray(dist, dtype=np.float64)
+        _l.check(self.lib.cup2d_amr_shape_set_dist(self._h, shape, dist.ctypes.data_as(C.POINTER(C.c_double))))
+
+    RIGID = ("u", "v", "omega", "center_of_mass", "M", "J", "length")
+
+    def collide(self, motions):
+        """the collision model (main.cpp:6705-6943) of shapes 0 .. len(motions)-1.  A motion is a mapping with u, v, omega (after
+        the 3x3 solve), center_of_mass, M, J and length.  Returns (uvw [N,3] after the model, sums [N,20] of main.cpp:6814-6837)"""
+        st = (_l.Rigid * len(motions))()
+        for k, m in enumerate(motions):
+            r = st[k]
+            r.u, r.v, r.omega = float(m["u"]), float(m["v"]), float(m["omega"])
+            r.center_of_mass[0], r.center_of_mass[1] = (float(x) for x in m["center_of_mass"])
+            r.M, r.J, r.length = float(m["M"]), float(m["J"]), float(m["length"])
+        sums = np.empty((len(motions), 20))
+        _l.check(self.lib.cup2d_amr_collide(self._h, len(motions), st, sums.ctypes.data_as(C.POINTER(C.c_double))))
+        return np.array([[r.u, r.v, r.omega] for r in st]).reshape(-1, 3), sums
+
     def close(self):
         if self._h:
             self.lib.cup2d_amr_destroy(self._h)

@@ -102,8 +102,9 @@ struct cup2d_amr {
   cup2d::GhostDev gt[3];            // compact ghost tables per stencil kind (cup2d_amr_plan_ghosts)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)
   // bodies (csrc/amr_penalize.cu): per-shape obstacle blocks, as cup2d_sim::Shape
-  // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid: csrc/amr_ongrid.cu)
-  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false; };
+  // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid or given one by cup2d_amr_shape_set_dist;
+  // ascending: the block ids are strictly ascending, recorded by cup2d_amr_shape_set, always true after cup2d_amr_ongrid)
+  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false, ascending = true; };
   std::vector<Shape> shapes;
   std::vector<int32_t> h_ij;        // [nb][2] block index (i, j) at the block's own level (filled by cup2d_amr_create)
   int *d_ij = nullptr;              // the same on the device (first use)
@@ -118,6 +119,11 @@ struct cup2d_amr {
   bool og_timing = false, og_timed = false; // cup2d_amr_ongrid_timing: CUDA events (cudaEvent_t) around the kernels of the last call
   void *og_ev[12] = {};
   void (*og_release)(cup2d_amr *) = nullptr; // destroys og_ev (set with them, csrc/amr_ongrid.cu)
+  // cup2d_amr_collide scratch (csrc/amr_collide.cu): staged shape / pair tables, per-pair matches, the 20 N sums
+  unsigned char *d_co_stage = nullptr;
+  int *d_co_match = nullptr;
+  double *d_co_sums = nullptr;
+  size_t co_stage_cap = 0, co_match_cap = 0, co_sums_cap = 0;
   void free_shapes() {
     for (auto &sh : shapes) {
       cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);
@@ -128,6 +134,9 @@ struct cup2d_amr {
     cudaFree(d_og_stage); cudaFree(d_og_part); cudaFree(d_og_mask); cudaFree(d_og_cnt);
     d_og_stage = d_og_part = nullptr, d_og_mask = nullptr, d_og_cnt = nullptr;
     og_stage_cap = og_part_cap = og_mask_cap = og_cnt_cap = 0;
+    cudaFree(d_co_stage); cudaFree(d_co_match); cudaFree(d_co_sums);
+    d_co_stage = nullptr, d_co_match = nullptr, d_co_sums = nullptr;
+    co_stage_cap = co_match_cap = co_sums_cap = 0;
     if (og_release) og_release(this);
     og_release = nullptr;
     og_timing = og_timed = false;

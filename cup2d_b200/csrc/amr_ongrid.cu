@@ -544,7 +544,7 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
       sh.cap = cap;
     }
     sh.nob = nob[s];
-    sh.has_dist = true;
+    sh.has_dist = sh.ascending = true;
     oids.ids[s] = sh.d_ids;
     pofs[s + 1] = pofs[s] + nob[s];
   }

@@ -31,7 +31,7 @@ SYMBOLS = [
     "cup2d_amr_peer_attach", "cup2d_peer_field_ptr", "cup2d_amr_dump", "cup2d_amr_create_ranks", "cup2d_amr_advect_diffuse_rhs_fast",
     "cup2d_amr_pressure_rhs_fast", "cup2d_amr_pressure_gradient_fast", "cup2d_amr_laplacian_fast", "cup2d_amr_set_fast",
     "cup2d_amr_adapt_mesh", "cup2d_amr_regrid", "cup2d_amr_ongrid", "cup2d_amr_shape_get",
-    "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times",
+    "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times", "cup2d_amr_shape_set_dist", "cup2d_amr_collide",
 ]
 
 
@@ -53,6 +53,12 @@ class Body(C.Structure):
     _fields_ = [("nm", C.c_int32), ("reserved", C.c_int32)] + [
         (n, C.POINTER(C.c_double)) for n in ("rX", "rY", "norX", "norY", "vX", "vY", "vNorX", "vNorY", "width")] + [
         ("center", C.c_double * 2), ("orientation", C.c_double), ("center_of_mass", C.c_double * 2)]
+
+
+class Rigid(C.Structure):
+    """cup2d_rigid: one shape's rigid motion and mass properties for the collision model (cup2d_amr_collide)"""
+    _fields_ = [("u", C.c_double), ("v", C.c_double), ("omega", C.c_double), ("center_of_mass", C.c_double * 2),
+                ("M", C.c_double), ("J", C.c_double), ("length", C.c_double)]
 
 
 _lib = None
@@ -163,6 +169,8 @@ def load_library():
     lib.cup2d_amr_ongrid_timing.argtypes = [P, I]
     lib.cup2d_amr_ongrid_times.argtypes = [P, C.POINTER(D)]
     lib.cup2d_amr_shape_get.argtypes = [P, I, C.POINTER(C.c_int32), C.POINTER(D), C.POINTER(D), C.POINTER(D)]
+    lib.cup2d_amr_shape_set_dist.argtypes = [P, I, C.POINTER(D)]
+    lib.cup2d_amr_collide.argtypes = [P, I, C.POINTER(Rigid), C.POINTER(D)]
     lib.cup2d_amr_create_ranks.argtypes = [L, C.POINTER(C.c_int32), I, I, D, D, I, I, C.POINTER(C.c_int64), I, C.POINTER(P)]
     lib.cup2d_amr_peer_export.argtypes = [P, P]
     lib.cup2d_amr_peer_attach.argtypes = [P, P]

@@ -125,7 +125,8 @@ int cup2d_dump(cup2d_sim *s, double time, const char *path);
  * order) with the shape's own chi[nob][8][8] and udef[nob][8][8][2].  Produced by the host body model every step. */
 int cup2d_shape_set(cup2d_sim *s, int shape, int nob, const int32_t *block_ids, const double *chi, const double *udef);
 /* main.cpp:6643-6688: out7 = {PM, PJ, PX, PY, UM, VM, AM}, summed over all ranks (every rank must call, also with
- * nob = 0).  The 3x3 solve for (u, v, omega) (6689-6703) and the collision model (6704-6943) stay on the host. */
+ * nob = 0).  The 3x3 solve for (u, v, omega) (6689-6703) stays on the host; the collision model (6704-6943) does too on
+ * this uniform context, and runs on the device for multi-level contexts (cup2d_amr_collide). */
 int cup2d_shape_integrals(cup2d_sim *s, int shape, double lambda, double dt, double cx, double cy, double *out7);
 /* main.cpp:6944-6979: vel = alpha vel + (1-alpha)(us - omega*py + udef_x, vs + omega*px + udef_y) on the cells the
  * shape owns (its chi > 0 and not below the chi field), alpha = 1/(1+lambda*dt) where its chi > 0.5.  Call per shape
@@ -359,7 +360,8 @@ int cup2d_amr_udef_assemble(cup2d_amr *a);
 
 /* ongrid() on a multi-level mesh (main.cpp:3991-4630; csrc/amr_ongrid.cu): the rasterisation of every body's midline into the
  * chi and tmp fields and into the shape's obstacle blocks, on the device.  The midline kinematics (main.cpp:4029-4207), the
- * 3x3 rigid-body solve, the collision model and ComputeSurfaceNormals stay with the caller. */
+ * 3x3 rigid-body solve and ComputeSurfaceNormals stay with the caller; the collision model reads the blocks on the device
+ * (cup2d_amr_collide). */
 typedef struct {
   int32_t nm, reserved;                /* midline points; nm >= 9 (Nsegments = (nm-1)/8 >= 1 dividing nm-1, main.cpp:4208-4210) */
   const double *rX, *rY, *norX, *norY; /* [nm] each: the shape-frame midline exactly as ongrid() holds it at main.cpp:4208 */
@@ -378,7 +380,7 @@ typedef struct {
  * aborts, 4009-4013); CUP2D_ESTATE for contexts on several ranks.  1 <= nshapes <= 64. */
 int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double *out);
 /* download shape k's obstacle blocks (any pointer may be NULL; returns nob): ids[nob], chi[nob][64], dist[nob][64] (shapes placed
- * by cup2d_amr_ongrid only), udef[nob][64][2] — what the host's collision model, forces and skins read */
+ * by cup2d_amr_ongrid or given by cup2d_amr_shape_set_dist), udef[nob][64][2] — what the host's forces and skins read */
 int cup2d_amr_shape_get(cup2d_amr *a, int shape, int32_t *ids, double *chi, double *dist, double *udef);
 /* CUDA-event timing of cup2d_amr_ongrid on the context's stream: timing(a, 1) creates the events and times every following call
  * (0 stops; a regrid clears it); times(a, ms8) gives the last timed call's milliseconds: {whole call on the stream (upload,
@@ -386,6 +388,28 @@ int cup2d_amr_shape_get(cup2d_amr *a, int shape, int32_t *ids, double *chi, doub
  * over the shapes */
 int cup2d_amr_ongrid_timing(cup2d_amr *a, int on);
 int cup2d_amr_ongrid_times(cup2d_amr *a, double *ms8);
+
+/* The collision model on a multi-level mesh (main.cpp:6705-6943 with collision() / compute_j() at 209-291; csrc/amr_collide.cu),
+ * on the obstacle blocks the device holds.  shape_set_dist uploads dist[nob][8][8] for a shape already set by
+ * cup2d_amr_shape_set (recorded or host-built shapes), which cup2d_amr_shape_get then returns; a later shape_set drops it. */
+int cup2d_amr_shape_set_dist(cup2d_amr *a, int shape, const double *dist);
+typedef struct {
+  double u, v, omega;       /* in: after the 3x3 solve (main.cpp:6699-6701); out: after the collision model (6937-6942) */
+  double center_of_mass[2]; /* Shape::centerOfMass */
+  double M, J, length;      /* Shape::M, Shape::J (cup2d_amr_ongrid's out[5], out[6]), Shape::length */
+} cup2d_rigid;
+/* Shapes 0 .. nshapes-1: over the cells of their common obstacle blocks where both chi are positive, each shape's sums of
+ * 6733-6813 (its own chi, chi pos, chi velocity, chi grad dist, then the same of its partners) on the device, added in the
+ * reference's order (partners in index order, blocks ascending, cells in row order), so bit-identical to the reference on one
+ * rank; then on the host the pair loop of 6863-6943 (both centroid masses >= 2, centroids within `length`, approaching) with
+ * the elastic impulse, which overwrites u, v, omega of both shapes of a pair.  Pairs are taken in (i ascending, j > i
+ * ascending) order, each seeing what earlier pairs left: the reference's result on one OpenMP thread.  With more than two
+ * shapes and several simultaneous collisions the reference's parallel loop has no defined order, and neither has its result.
+ * sums20 (may be NULL) gets [nshapes][20] in the layout of 6814-6837 (the Z slots zero).  Fields and shape data are not
+ * changed.  CUP2D_EINVAL for nshapes outside 1..64, a shape not set or one whose block ids are not strictly ascending
+ * (cup2d_amr_ongrid leaves them ascending); CUP2D_ESTATE for a shape without dist or a context on several ranks.  On any
+ * error `shapes` and the context are untouched. */
+int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *sums20);
 
 #ifdef __cplusplus
 }

@@ -6,6 +6,7 @@ reference grows for its run.sh case (config C5 of SURVEY 8(d) at the chosen leve
       under torchrun on N GPUs: the mesh distributed by block ranges, cup2d_amr_create_ranks)
   python tools/bench_amr.py regrid [base_level=9]      one adapt() of the C5 mesh: decision, regrid, transfer kernels
   python tools/bench_amr.py ongrid [base_level=9]      cup2d_amr_ongrid of two fish in the finest region of the C5 mesh
+  python tools/bench_amr.py collide [base_level=9]     cup2d_amr_collide of two overlapping fish there, after ongrid
 
 The mesh comes from oracle/_ref/ref_harness amrlab (which travels to the GPU box prebuilt), the fields are its seeded ones,
 bodies are left out (u_def = 0, chi = 0).  Prints one JSON line: blocks, cells, levels, ms per step with CUDA events on the
@@ -203,7 +204,62 @@ def ongrid(base, reps=20):
     sim.close()
 
 
+def collide(base, reps=20):
+    """cup2d_amr_collide of two run.sh-sized fish (as in ongrid above) placed to overlap along most of their length in the
+    finest region of the C5 mesh, after ongrid: the call timed with CUDA events (median over the calls; recorded on the
+    legacy default stream, which the context's blocking stream is ordered with, so they bracket the upload, both kernels, the
+    download and the host's pair loop), the host wall time per call, and the PCIe bytes per step the call removes (every
+    shape's ids, chi, dist and u_def that a host collision model would download)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import torch
+    import amr_body_oracle as bo
+    from cup2d_b200.amr import AmrSimulation
+    blocks = three_level_mesh(base)
+    h0 = 1.0 / 8
+    hmin = h0 / (1 << int(blocks[:, 0].max()))
+    L = 0.05
+    nm = 8 * int(np.ceil(L / (hmin / np.sqrt(2)) / 8)) + 1
+    bodies = [bo.synthetic_body((0.48, 0.52), L, nm, 0.2), bo.synthetic_body((0.4802, 0.5204), L, nm, 0.25, phase=1.0)]
+    sim = AmrSimulation(blocks, 1, 1, h0, 1e-4)
+    out = sim.ongrid(bodies)
+    motions = [{"u": 0.1 - 0.2 * k, "v": 0.05 - 0.1 * k, "omega": 0.3 - 0.6 * k, "center_of_mass": out[k, 3:5], "M": out[k, 5],
+                "J": out[k, 6], "length": L} for k in range(2)]
+    for _ in range(3):
+        uvw, sums = sim.collide(motions)
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        sim.collide(motions)
+    t_wall = (time.perf_counter() - t0) / reps
+    ms = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        sim.collide(motions)
+        e1.record()
+        e1.synchronize()
+        ms.append(e0.elapsed_time(e1))
+    ids = [sim.shape_get(k, dist=False)["ids"] for k in range(2)]
+    nob = [len(i) for i in ids]
+    props = torch.cuda.get_device_properties(0)
+    try:
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                               text=True).stdout.strip()
+    except Exception:
+        power = "unknown"
+    print(json.dumps({"workload": f"collide of two overlapping fish (Nm {nm}) on the synthetic 3-level mesh, base level {base}",
+                      "blocks": len(blocks), "obstacle_blocks": nob, "common_blocks": len(np.intersect1d(*ids)),
+                      "iM": sums[:, 0].tolist(), "t_call_events_ms_median": float(np.median(ms)),
+                      "t_call_events_ms_min": float(np.min(ms)), "t_call_wall_ms": t_wall * 1e3,
+                      "pcie_bytes_removed_per_step": sum(nob) * (4 + 64 * 8 + 64 * 8 + 128 * 8),
+                      "uvw_after": uvw.tolist(), "gpu": props.name, "power_limit": power}))
+    sim.close()
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "collide":     # python tools/bench_amr.py collide [base_level=9]
+        collide(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "ongrid":      # python tools/bench_amr.py ongrid [base_level=9]
         ongrid(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
         return
