@@ -99,6 +99,40 @@ assert worst < 1e-12
     assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
 
 
+def test_krylov_restart_on_three_ranks_emulated(emulated_library):
+    """the BiCGSTAB breakdown restart on several ranks (tests/krylov_cases.py:restart_on_ranks): 6x4 blocks split over three
+    ranks as threads of one process, so k_pupdate pushes p = r and z = M p to the peers and every rank decides the restart
+    and the restart cap on all-reduced sums.  max_restarts 1 and 100: every rank stops at the one-rank count (the breakdown
+    iteration, and breakdown + 6), and the assembled iterate is the one-rank iterate to 1e-10"""
+    code = r'''
+import sys, threading
+sys.path[:0] = [%r, %r, %r]
+import krylov_cases as kc
+W = 3
+bar, slots, res, errs = threading.Barrier(W), [None] * W, [None] * W, []
+class Dist:
+    def __init__(self, rank): self.rank = rank
+    def all_gather_object(self, out, obj):
+        slots[self.rank] = obj; bar.wait(); out[:] = slots; bar.wait()
+    def barrier(self): bar.wait()
+def run(rank):
+    try:
+        res[rank] = kc.restart_on_ranks(rank, W, Dist(rank))
+    except Exception as e:
+        errs.append(repr(e)); bar.abort()
+ths = [threading.Thread(target=run, args=(r,)) for r in range(W)]
+[t.start() for t in ths]; [t.join() for t in ths]
+assert not errs, errs
+one = kc.restart_on_ranks(0, 1, None)
+bd = kc.uniform_breakdown(*kc.BREAKDOWNS[0][0], *kc.BREAKDOWNS[0][1:])
+assert one[1][0] == bd["k"] and one[100][0] == bd["kmax"], (one[1][0], one[100][0])
+print("WORST", kc.check_ranks(res, one))
+''' % (ROOT, HERE, os.path.join(ROOT, "oracle"))
+    r = subprocess.run([sys.executable, "-c", code], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600,
+                       env=dict(os.environ, CUP2D_B200_LIB=emulated_library))
+    assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
+
+
 def test_a_rank_that_never_arrives_fails_the_call_instead_of_hanging(emulated_library):
     """bounded cross-GPU waits: rank 1 attaches but never issues its step; rank 0's first halo wait runs into the time limit
     (CUP2D_COMM_TIMEOUT_MS), every later wait is skipped, and the call that synchronises reports CUP2D_ECOMM — the reference

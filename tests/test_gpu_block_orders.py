@@ -177,18 +177,18 @@ def neighbour_table(sim):
     return nbr
 
 
-def five_kernel_solve(nbr, b_blocks, K):
-    """K iterations of the five-kernel BiCGSTAB (a Poisson-only context always runs it) from x0 = 0"""
+def five_kernel_solve(nbr, b_blocks, K, x0_blocks=None, tol_abs=0.0, tol_rel=0.0, max_restarts=0):
+    """at most K iterations of the five-kernel BiCGSTAB (a Poisson-only context always runs it) from x0 (default 0)"""
     lib = cup2d_b200.load_library()
     h = C.c_void_p()
     nblk = len(nbr) // 4
     Lb.check(lib.cup2d_poisson_create(nblk, nbr.ctypes.data_as(C.POINTER(C.c_int32)), 0, C.byref(h)))
     try:
-        x = np.zeros_like(b_blocks)
+        x = np.zeros_like(b_blocks) if x0_blocks is None else np.array(x0_blocks, dtype=np.float64)
         Lb.check(lib.cup2d_field_upload(h, Lb.FIELDS["tmp"], b_blocks.ctypes.data))
         Lb.check(lib.cup2d_field_upload(h, Lb.FIELDS["pres"], x.ctypes.data))
         it, err = C.c_int(), C.c_double()
-        Lb.check(lib.cup2d_poisson_solve(h, 0.0, 0.0, 0, K, C.byref(it), C.byref(err)))
+        Lb.check(lib.cup2d_poisson_solve(h, tol_abs, tol_rel, max_restarts, K, C.byref(it), C.byref(err)))
         Lb.check(lib.cup2d_field_download(h, Lb.FIELDS["pres"], x.ctypes.data))
     finally:
         lib.cup2d_destroy(h)
