@@ -8,7 +8,8 @@ import numpy as np
 from . import lib as _l
 
 LAB_SHAPES = {0: (14, 14, 2), 1: (10, 10, 2), 2: (10, 10, 1), 3: (16, 16, 1),  # kind 3: chi lab of GradChiOnTmp
-              4: (10, 10, 2), 5: (10, 10, 1)}  # kinds 4, 5: the +-1 labs with corners that adapt() refines from
+              4: (10, 10, 2), 5: (10, 10, 1),  # kinds 4, 5: the +-1 labs with corners that adapt() refines from
+              6: (16, 16, 2)}  # kind 6: velocity lab of the force diagnostics
 
 
 def adapt_mesh(blocks, bpdx, bpdy, level_max, block_linf, rtol, ctol):
@@ -341,6 +342,46 @@ class AmrSimulation:
         sums = np.empty((len(motions), 20))
         _l.check(self.lib.cup2d_amr_collide(self._h, len(motions), st, sums.ctypes.data_as(C.POINTER(C.c_double))))
         return np.array([[r.u, r.v, r.omega] for r in st]).reshape(-1, 3), sums
+
+    # ---- surface normals and force diagnostics on the device (cup2d_amr_surface / _surface_get / _forces) ----
+    def surface(self, n):
+        """ComputeSurfaceNormals (main.cpp:3774-3828) of shapes 0 .. n-1 on chi and tmp as they stand (after ongrid)"""
+        _l.check(self.lib.cup2d_amr_surface(self._h, int(n)))
+
+    SKIN = ("x_s", "y_s", "p_s", "u_s", "v_s", "nx_s", "ny_s", "omega_s", "uDef_s", "vDef_s", "fX_s", "fY_s", "fXv_s", "fYv_s")
+
+    def surface_get(self, shape):
+        """shape `shape`'s surface points: dict of block [n] (block ids), ixy [n, 2], normal [n, 3] = (dchidx, dchidy, D) and
+        skin [n, 14] (the columns of SKIN, of the last forces call; zero before)"""
+        n = self.lib.cup2d_amr_surface_get(self._h, int(shape), None, None, None, None)
+        if n < 0:
+            _l.check(int(n))
+        blk, ixy, nrm, skin = np.empty(n, dtype=np.int32), np.empty((n, 2), dtype=np.int32), np.empty((n, 3)), np.empty((n, 14))
+        P, I32 = C.POINTER(C.c_double), C.POINTER(C.c_int32)
+        rc = self.lib.cup2d_amr_surface_get(self._h, int(shape), blk.ctypes.data_as(I32), ixy.ctypes.data_as(I32),
+                                            nrm.ctypes.data_as(P), skin.ctypes.data_as(P))
+        if rc < 0:
+            _l.check(int(rc))
+        return {"block": blk, "ixy": ixy, "normal": nrm, "skin": skin}
+
+    FORCES = ("circulation", "perimeter", "forcex", "forcex_P", "forcex_V", "torque_P", "drag", "lift", "Pout", "PoutNew",
+              "PoutBnd", "torque", "forcey", "forcey_P", "forcey_V", "torque_V", "thrust", "defPowerBnd", "defPower",
+              "Pthrust", "Pdrag", "EffPDef", "EffPDefBnd")
+
+    def forces(self, motions):
+        """KernelComputeForces and its reductions (main.cpp:5573-5746, 7188-7284) for shapes 0 .. len(motions)-1 from vel,
+        pres, chi and each shape's u_def.  A motion is a mapping as for collide (u, v and center_of_mass are read).  Returns
+        [N, 23] with the columns of FORCES"""
+        st = (_l.Rigid * len(motions))()
+        for k, m in enumerate(motions):
+            r = st[k]
+            r.u, r.v = float(m["u"]), float(m["v"])
+            r.omega = float(m.get("omega", 0.0))
+            r.center_of_mass[0], r.center_of_mass[1] = (float(x) for x in m["center_of_mass"])
+            r.M, r.J, r.length = (float(m.get(n, 0.0)) for n in ("M", "J", "length"))
+        out = np.empty((len(motions), 23))
+        _l.check(self.lib.cup2d_amr_forces(self._h, len(motions), st, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
 
     def close(self):
         if self._h:

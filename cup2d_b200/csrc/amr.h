@@ -99,12 +99,15 @@ struct cup2d_amr {
   int *d_nbr4 = nullptr;            // [nb][4] W,E,S,N: same-level block, -1 wall, -2 coarser/finer
   int *d_irr_of = nullptr;          // [nb] position in the irregular list or -1
   int64_t nirr = 0;
-  cup2d::GhostDev gt[3];            // compact ghost tables per stencil kind (cup2d_amr_plan_ghosts)
+  cup2d::GhostDev gt[7];            // compact ghost tables per stencil kind (cup2d_amr_plan_ghosts): 0-2 with the fast tables,
+                                    // 3 and 6 (the force diagnostics' labs, csrc/amr_forces.cu) on first use
+  int *d_nbr8 = nullptr;            // [nb][8] cup2d_amr_plan_neighbours on the device (csrc/amr_forces.cu, first use)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)
   // bodies (csrc/amr_penalize.cu): per-shape obstacle blocks, as cup2d_sim::Shape
   // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid or given one by cup2d_amr_shape_set_dist;
   // ascending: the block ids are strictly ascending, recorded by cup2d_amr_shape_set, always true after cup2d_amr_ongrid)
-  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false, ascending = true; };
+  // (has_surface: cup2d_amr_surface has run on the shape as it stands; cup2d_amr_shape_set and cup2d_amr_ongrid clear it)
+  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false, ascending = true, has_surface = false; };
   std::vector<Shape> shapes;
   std::vector<int32_t> h_ij;        // [nb][2] block index (i, j) at the block's own level (filled by cup2d_amr_create)
   int *d_ij = nullptr;              // the same on the device (first use)
@@ -124,6 +127,12 @@ struct cup2d_amr {
   int *d_co_match = nullptr;
   double *d_co_sums = nullptr;
   size_t co_stage_cap = 0, co_match_cap = 0, co_sums_cap = 0;
+  // cup2d_amr_surface / cup2d_amr_forces (csrc/amr_forces.cu): per shape the surface points of its obstacle blocks, 64 slots
+  // per block (slot k * 64 + j = point j of block k): (ix, iy), {dchidx, dchidy, D}, the 14 skin values; counts per block
+  struct Surface { int cap = 0; int *d_ixy = nullptr, *d_cnt = nullptr; double *d_nrm = nullptr, *d_skin = nullptr; std::vector<int> cnt; };
+  std::vector<Surface> surf;
+  double *d_fo_part = nullptr;      // [obstacle blocks][19] per-block accumulators, then [nshapes][19] sums
+  size_t fo_part_cap = 0;
   void free_shapes() {
     for (auto &sh : shapes) {
       cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);
@@ -137,6 +146,12 @@ struct cup2d_amr {
     cudaFree(d_co_stage); cudaFree(d_co_match); cudaFree(d_co_sums);
     d_co_stage = nullptr, d_co_match = nullptr, d_co_sums = nullptr;
     co_stage_cap = co_match_cap = co_sums_cap = 0;
+    for (auto &q : surf) {
+      cudaFree(q.d_ixy); cudaFree(q.d_cnt); cudaFree(q.d_nrm); cudaFree(q.d_skin);
+    }
+    surf.clear();
+    cudaFree(d_fo_part);
+    d_fo_part = nullptr, fo_part_cap = 0;
     if (og_release) og_release(this);
     og_release = nullptr;
     og_timing = og_timed = false;

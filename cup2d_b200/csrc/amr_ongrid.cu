@@ -545,6 +545,7 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
     }
     sh.nob = nob[s];
     sh.has_dist = sh.ascending = true;
+    sh.has_surface = false;
     oids.ids[s] = sh.d_ids;
     pofs[s + 1] = pofs[s] + nob[s];
   }

@@ -424,7 +424,7 @@ void cup2d_amr_destroy(cup2d_amr *a) {
   }
   for (auto p : a->lab) cudaFree(p);
   cudaFree(a->lab_udef); cudaFree(a->d_h); cudaFree(a->d_cf[0]); cudaFree(a->d_cf[1]); cudaFree(a->d_part);
-  cudaFree(a->d_nbr4); cudaFree(a->d_irr_of); cudaFree(a->d_faceflux);
+  cudaFree(a->d_nbr4); cudaFree(a->d_nbr8); cudaFree(a->d_irr_of); cudaFree(a->d_faceflux);
   a->free_shapes();
   for (auto &g : a->gt) {
     cudaFree(g.grow); cudaFree(g.rowptr); cudaFree(g.dst); cudaFree(g.sb); cudaFree(g.sc); cudaFree(g.w);

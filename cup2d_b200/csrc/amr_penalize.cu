@@ -165,6 +165,7 @@ int cup2d_amr_shape_set(cup2d_amr *a, int shape, int nob, const int32_t *block_i
   if ((int)a->shapes.size() <= shape) a->shapes.resize(shape + 1);
   cup2d_amr::Shape &sh = a->shapes[shape];
   sh.has_dist = false;
+  sh.has_surface = false;
   sh.ascending = true; // what cup2d_amr_collide needs of the ids (recorded, not enforced here)
   for (int k = 1; k < nob; k++) sh.ascending = sh.ascending && block_ids[k - 1] < block_ids[k];
   if (nob > sh.cap) {

@@ -121,6 +121,8 @@ struct LabBuilder {
     // 4, 5: the labs adapt() refines a block from (main.cpp:4908-4967): +-1 with corners, vector / scalar wall rules
     else if (which == 4) { dim = 2; sx = sy = -1; ex = ey = 2; tens = true; vector_bc = true; }
     else if (which == 5) { dim = 1; sx = sy = -1; ex = ey = 2; tens = true; vector_bc = false; }
+    // 6: KernelComputeForces's velocity lab (main.cpp:5576, 7188): +-4 with corners, vector wall rule
+    else if (which == 6) { dim = 2; sx = sy = -4; ex = ey = 5; tens = true; vector_bc = true; }
     else { dim = 1; sx = sy = -4; ex = ey = 5; tens = true; vector_bc = false; } // GradChiOnTmp's chi lab (main.cpp:4633)
     nmx = BS + ex - sx - 1, nmy = BS + ey - sy - 1;
     ox = cdiv(sx - 1, 2) - 1, oy = cdiv(sy - 1, 2) - 1;
@@ -405,14 +407,14 @@ struct GhostTable { // compact form: ghost rows of irregular blocks only
 struct cup2d_amr_plan {
   Mesh mesh;
   std::vector<int32_t> irregular; // blocks with a coarser or finer block among their 8 neighbours
-  GhostTable ghosts[4];
+  GhostTable ghosts[7];                          // kinds 0-3 and 6
   // CSR per stencil kind: rows = (block, iy, ix, comp)
-  std::vector<int64_t> rowptr[6];
-  std::vector<int32_t> src_block[6], src_cc[6]; // source block, source cell*dim + comp
-  std::vector<double> w[6];
+  std::vector<int64_t> rowptr[7];
+  std::vector<int32_t> src_block[7], src_cc[7]; // source block, source cell*dim + comp
+  std::vector<double> w[7];
   // coarse-fine faces: (fine block, fine face, coarse block, coarse face, half)
   std::vector<int32_t> faces;
-  bool built[6] = {false, false, false, false, false, false};
+  bool built[7] = {false, false, false, false, false, false, false};
 };
 
 // full lab rows of the blocks `ks` (in that order) for stencil kind `which`, appended to the CSR (rp, sb, sc, w)
@@ -452,7 +454,7 @@ const std::vector<int> &amr_plan_level_ij(const cup2d_amr_plan *p, int *bpdx, in
 // table of the whole mesh
 int amr_plan_subset_rows(cup2d_amr_plan *p, int which, int64_t nsub, const int32_t *blocks, std::vector<int64_t> &rowptr,
                          std::vector<int32_t> &src_block, std::vector<int32_t> &src_cellcomp, std::vector<double> &weight) {
-  if (!p || which < 0 || which > 5 || nsub < 0) return CUP2D_EINVAL;
+  if (!p || which < 0 || which > 6 || nsub < 0) return CUP2D_EINVAL;
   const int64_t n = (int64_t)p->mesh.lij.size() / 3;
   for (int64_t q = 0; q < nsub; q++)
     if (blocks[q] < 0 || blocks[q] >= n) return CUP2D_EINVAL;
@@ -699,7 +701,7 @@ int64_t cup2d_amr_plan_irregular(cup2d_amr_plan *p, int32_t *out) {
 
 int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int64_t *rowptr, int32_t *dst, int32_t *src_block,
                               int32_t *src_cellcomp, double *weight) {
-  if (!p || which < 0 || which > 3) return CUP2D_EINVAL;
+  if (!p || which < 0 || (which > 3 && which != 6)) return CUP2D_EINVAL;
   GhostTable &g = p->ghosts[which];
   if (!g.built) build_ghosts(p, which);
   const int64_t nnz = (int64_t)g.w.size();
@@ -714,7 +716,7 @@ int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int6
 
 int64_t cup2d_amr_plan_stencil(cup2d_amr_plan *p, int which, int64_t *rowptr, int32_t *src_block, int32_t *src_cellcomp,
                                double *weight) {
-  if (!p || which < 0 || which > 5) return CUP2D_EINVAL;
+  if (!p || which < 0 || which > 6) return CUP2D_EINVAL;
   if (!p->built[which]) build(p, which);
   const int64_t nnz = (int64_t)p->w[which].size();
   if (rowptr) memcpy(rowptr, p->rowptr[which].data(), p->rowptr[which].size() * sizeof(int64_t));
@@ -849,7 +851,7 @@ int64_t cup2d_amr_plan_poisson(cup2d_amr_plan *p, int32_t *nbr_out, int64_t *nnz
 
 /* bookkeeping of the last cup2d_amr_plan_ghosts(which): distinct local configurations, directly evaluated blocks */
 int cup2d_amr_plan_stats(cup2d_amr_plan *p, int which, int32_t *npatterns, int32_t *fallbacks) {
-  if (!p || which < 0 || which > 3 || !p->ghosts[which].built) return CUP2D_EINVAL;
+  if (!p || which < 0 || (which > 3 && which != 6) || !p->ghosts[which].built) return CUP2D_EINVAL;
   if (npatterns) *npatterns = p->ghosts[which].npatterns;
   if (fallbacks) *fallbacks = p->ghosts[which].fallbacks;
   return CUP2D_OK;

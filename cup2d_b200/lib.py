@@ -32,6 +32,7 @@ SYMBOLS = [
     "cup2d_amr_pressure_rhs_fast", "cup2d_amr_pressure_gradient_fast", "cup2d_amr_laplacian_fast", "cup2d_amr_set_fast",
     "cup2d_amr_adapt_mesh", "cup2d_amr_regrid", "cup2d_amr_ongrid", "cup2d_amr_shape_get",
     "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times", "cup2d_amr_shape_set_dist", "cup2d_amr_collide",
+    "cup2d_amr_surface", "cup2d_amr_surface_get", "cup2d_amr_forces",
 ]
 
 
@@ -171,6 +172,10 @@ def load_library():
     lib.cup2d_amr_shape_get.argtypes = [P, I, C.POINTER(C.c_int32), C.POINTER(D), C.POINTER(D), C.POINTER(D)]
     lib.cup2d_amr_shape_set_dist.argtypes = [P, I, C.POINTER(D)]
     lib.cup2d_amr_collide.argtypes = [P, I, C.POINTER(Rigid), C.POINTER(D)]
+    lib.cup2d_amr_surface.argtypes = [P, I]
+    lib.cup2d_amr_surface_get.argtypes = [P, I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(D), C.POINTER(D)]
+    lib.cup2d_amr_surface_get.restype = L
+    lib.cup2d_amr_forces.argtypes = [P, I, C.POINTER(Rigid), C.POINTER(D)]
     lib.cup2d_amr_create_ranks.argtypes = [L, C.POINTER(C.c_int32), I, I, D, D, I, I, C.POINTER(C.c_int64), I, C.POINTER(P)]
     lib.cup2d_amr_peer_export.argtypes = [P, P]
     lib.cup2d_amr_peer_attach.argtypes = [P, P]

@@ -238,7 +238,9 @@ typedef struct cup2d_amr_plan cup2d_amr_plan;
 int cup2d_amr_plan_create(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, cup2d_amr_plan **out);
 void cup2d_amr_plan_destroy(cup2d_amr_plan *p);
 /* which: 0 = velocity lab of the advect stencil {-3,-3,4,4,tensorial} (14x14x2 per block), 1 = velocity lab of the
- * +-1 stencil (10x10x2), 2 = scalar lab of the +-1 stencil (10x10).  Rows = (block, iy, ix, comp) in that order; row r
+ * +-1 stencil (10x10x2), 2 = scalar lab of the +-1 stencil (10x10), 3 = scalar lab {-4,-4,5,5,tensorial} (16x16), 4 / 5 =
+ * vector / scalar labs of the +-1 stencil with corners, 6 = velocity lab {-4,-4,5,5,tensorial} of the force diagnostics
+ * (16x16x2).  Rows = (block, iy, ix, comp) in that order; row r
  * is sum_e weight[e] * field[src_block[e]][src_cellcomp[e]] (cell*dim + comp of the source block).  A row without
  * entries is a lab cell the reference never writes (corner ghosts of the non-tensorial stencils).  Returns nnz; any
  * output pointer may be NULL (call once to size, once to fill; rowptr has nrows + 1 entries). */
@@ -252,6 +254,7 @@ int64_t cup2d_amr_plan_stencil(cup2d_amr_plan *p, int which, int64_t *rowptr, in
 int64_t cup2d_amr_plan_irregular(cup2d_amr_plan *p, int32_t *blocks_out);
 int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int64_t *rowptr, int32_t *dst,
                               int32_t *src_block, int32_t *src_cellcomp, double *weight);
+/* (cup2d_amr_plan_ghosts and cup2d_amr_plan_stats take the kinds 0-3 and 6) */
 /* ghost tables are instantiated from a dictionary of local configurations (blocks with the same neighbourhood share one
  * symbolically evaluated pattern); after cup2d_amr_plan_ghosts(which): how many patterns, how many blocks bypassed it */
 int cup2d_amr_plan_stats(cup2d_amr_plan *p, int which, int32_t *npatterns, int32_t *fallbacks);
@@ -360,8 +363,8 @@ int cup2d_amr_udef_assemble(cup2d_amr *a);
 
 /* ongrid() on a multi-level mesh (main.cpp:3991-4630; csrc/amr_ongrid.cu): the rasterisation of every body's midline into the
  * chi and tmp fields and into the shape's obstacle blocks, on the device.  The midline kinematics (main.cpp:4029-4207), the
- * 3x3 rigid-body solve and ComputeSurfaceNormals stay with the caller; the collision model reads the blocks on the device
- * (cup2d_amr_collide). */
+ * 3x3 rigid-body solve stay with the caller; the collision model (cup2d_amr_collide), the surface normals (cup2d_amr_surface)
+ * and the force diagnostics (cup2d_amr_forces) read the blocks on the device. */
 typedef struct {
   int32_t nm, reserved;                /* midline points; nm >= 9 (Nsegments = (nm-1)/8 >= 1 dividing nm-1, main.cpp:4208-4210) */
   const double *rX, *rY, *norX, *norY; /* [nm] each: the shape-frame midline exactly as ongrid() holds it at main.cpp:4208 */
@@ -410,6 +413,30 @@ typedef struct {
  * (cup2d_amr_ongrid leaves them ascending); CUP2D_ESTATE for a shape without dist or a context on several ranks.  On any
  * error `shapes` and the context are untouched. */
 int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *sums20);
+
+/* Surface normals and force diagnostics on a multi-level mesh (csrc/amr_forces.cu), on the obstacle blocks the device holds:
+ * what a caller otherwise computes on the host from downloaded vel, pres and chi.  Bit-identical to the reference on one rank
+ * where the labs involved are copies (no level jump); elsewhere the labs come from the plan's ghost rows, to rounding.
+ * ComputeSurfaceNormals (main.cpp:3774-3828, as ongrid() calls it at 4470) on the chi and tmp fields as they stand, for shapes
+ * 0 .. nshapes-1: each obstacle block's surface points (ix, iy, dchidx, dchidy, D) in the reference's push order.  Call it
+ * after cup2d_amr_ongrid and before anything overwrites tmp (poisson_rhs, adapt_tags), as the reference does.  The reference
+ * reads its lab rows there without their offset, so three cells per block read a corner ghost no rule writes; those hold
+ * chi = 0 and tmp = -1, the reference's values while the bodies are away from the domain walls.  cup2d_amr_shape_set,
+ * cup2d_amr_ongrid and cup2d_amr_regrid drop the points.  CUP2D_EINVAL for nshapes outside 1..64 or a shape not set;
+ * CUP2D_ESTATE for contexts on several ranks. */
+int cup2d_amr_surface(cup2d_amr *a, int nshapes);
+/* shape k's surface points: block[n] (block id), ixy[n][2], normal[n][3] = {dchidx, dchidy, D}; skin[n][14] = x_s, y_s, p_s,
+ * u_s, v_s, nx_s, ny_s, omega_s, uDef_s, vDef_s, fX_s, fY_s, fXv_s, fYv_s of the last cup2d_amr_forces call (zero before).
+ * Any pointer may be NULL; returns n (CUP2D_EINVAL: no such shape, CUP2D_ESTATE: no points since the shape was last set). */
+int64_t cup2d_amr_surface_get(cup2d_amr *a, int shape, int32_t *block, int32_t *ixy, double *normal, double *skin);
+/* KernelComputeForces + main.cpp:7188-7284 from vel, pres, chi and each shape's u_def: out[23*k ..] = quantities[0..18] in the
+ * order of 7233-7251 (circulation, perimeter, forcex, forcex_P, forcex_V, torque_P, drag, lift, Pout, PoutNew, PoutBnd, torque,
+ * forcey, forcey_P, forcey_V, torque_V, thrust, defPowerBnd, defPower), then Pthrust, Pdrag, EffPDef, EffPDefBnd (7273-7280).
+ * Reads u, v and center_of_mass of shapes[k] (cup2d_rigid, as cup2d_amr_collide leaves them).  Points, then blocks in
+ * ascending id order, are added as the reference's serial chains.  Fields and shape data are not changed.  CUP2D_EINVAL for
+ * nshapes outside 1..64, a shape not set or a NULL shapes / out; CUP2D_ESTATE for a shape whose surface points were dropped
+ * or a context on several ranks.  On any error the context and out are untouched. */
+int cup2d_amr_forces(cup2d_amr *a, int nshapes, const cup2d_rigid *shapes, double *out);
 
 #ifdef __cplusplus
 }

@@ -7,6 +7,7 @@ reference grows for its run.sh case (config C5 of SURVEY 8(d) at the chosen leve
   python tools/bench_amr.py regrid [base_level=9]      one adapt() of the C5 mesh: decision, regrid, transfer kernels
   python tools/bench_amr.py ongrid [base_level=9]      cup2d_amr_ongrid of two fish in the finest region of the C5 mesh
   python tools/bench_amr.py collide [base_level=9]     cup2d_amr_collide of two overlapping fish there, after ongrid
+  python tools/bench_amr.py forces [base_level=9]      cup2d_amr_surface + cup2d_amr_forces of the same two fish, seeded vel, pres
 
 The mesh comes from oracle/_ref/ref_harness amrlab (which travels to the GPU box prebuilt), the fields are its seeded ones,
 bodies are left out (u_def = 0, chi = 0).  Prints one JSON line: blocks, cells, levels, ms per step with CUDA events on the
@@ -256,7 +257,69 @@ def collide(base, reps=20):
     sim.close()
 
 
+def forces(base, reps=20):
+    """cup2d_amr_surface and cup2d_amr_forces of the two fish of `collide` above, after ongrid, with seeded vel and pres: each
+    call timed with CUDA events (median over the calls; recorded on the legacy default stream, which the context's blocking
+    stream is ordered with), the host wall time per call, the surface points and obstacle blocks, and the PCIe bytes per step
+    the calls remove (vel, pres and chi that host force diagnostics would download: 32 B per cell)"""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import torch
+    import amr_body_oracle as bo
+    from cup2d_b200.amr import AmrSimulation
+    blocks = three_level_mesh(base)
+    h0 = 1.0 / 8
+    hmin = h0 / (1 << int(blocks[:, 0].max()))
+    L = 0.05
+    nm = 8 * int(np.ceil(L / (hmin / np.sqrt(2)) / 8)) + 1
+    bodies = [bo.synthetic_body((0.48, 0.52), L, nm, 0.2), bo.synthetic_body((0.4802, 0.5204), L, nm, 0.25, phase=1.0)]
+    sim = AmrSimulation(blocks, 1, 1, h0, 1e-4)
+    out = sim.ongrid(bodies)
+    vel, pres = seeded_fields(blocks, h0)
+    sim.upload("vel", vel)
+    sim.upload("pres", pres)
+    motions = [{"u": 0.1 - 0.2 * k, "v": 0.05 - 0.1 * k, "center_of_mass": out[k, 3:5]} for k in range(2)]
+
+    def timed(f):
+        for _ in range(3):
+            f()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            f()
+        t_wall = (time.perf_counter() - t0) / reps
+        ms = []
+        for _ in range(reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            f()
+            e1.record()
+            e1.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        return float(np.median(ms)), t_wall * 1e3
+    ms_s, wall_s = timed(lambda: sim.surface(2))
+    ms_f, wall_f = timed(lambda: sim.forces(motions))
+    res = sim.forces(motions)
+    npts = [len(sim.surface_get(k)["block"]) for k in range(2)]
+    nob = [len(sim.shape_get(k, dist=False)["ids"]) for k in range(2)]
+    props = torch.cuda.get_device_properties(0)
+    try:
+        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                               text=True).stdout.strip()
+    except Exception:
+        power = "unknown"
+    print(json.dumps({"workload": f"surface + forces of two overlapping fish (Nm {nm}) on the synthetic 3-level mesh, base level {base}",
+                      "blocks": len(blocks), "obstacle_blocks": nob, "surface_points": npts,
+                      "t_surface_events_ms_median": ms_s, "t_surface_wall_ms": wall_s,
+                      "t_forces_events_ms_median": ms_f, "t_forces_wall_ms": wall_f,
+                      "pcie_bytes_removed_per_step": len(blocks) * 64 * 32, "forcex": res[:, 2].tolist(), "forcey": res[:, 12].tolist(),
+                      "gpu": props.name, "power_limit": power}))
+    sim.close()
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "forces":      # python tools/bench_amr.py forces [base_level=9]
+        forces(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
+        return
     if len(sys.argv) > 1 and sys.argv[1] == "collide":     # python tools/bench_amr.py collide [base_level=9]
         collide(int(sys.argv[2]) if len(sys.argv) > 2 else 9)
         return
