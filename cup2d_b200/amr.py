@@ -271,6 +271,10 @@ class AmrSimulation:
     def udef_assemble(self):
         _l.check(self.lib.cup2d_amr_udef_assemble(self._h))
 
+    def udef_blend(self):
+        """vel = vel (1 - chi) + tmpV chi, the blend before the reference's time loop (main.cpp:6566-6575)"""
+        _l.check(self.lib.cup2d_amr_udef_blend(self._h))
+
     # ---- ongrid() on the device (cup2d_amr_ongrid) ----
     MIDLINE = ("rX", "rY", "norX", "norY", "vX", "vY", "vNorX", "vNorY", "width")
 

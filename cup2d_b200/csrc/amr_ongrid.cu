@@ -16,6 +16,7 @@
 //                              kind-2 ghost rows at level jumps); per-block Mass / COM partials, summed cell by cell in order
 //   amr_ongrid_moments_kernel  the seven sums of 4489-4518 per block, cell by cell in order
 //   amr_ongrid_correct_kernel  udef -= (u - a py, v + a px) (4541-4556)
+//   amr_udef_blend_kernel      cup2d_amr_udef_blend: vel = vel (1 - chi) + tmpV chi before the time loop (6566-6575)
 // The host adds the per-block partials in block order (as cup2d_amr_shape_integrals does).  This file is compiled without FMA
 // contraction (Makefile), like the reference (-O3, no -ffp-contract=fast on x86-64), so every expression rounds as it does there.
 #include "sim.h"
@@ -436,6 +437,17 @@ static void og_segment(const cup2d_body &B, int idx, int next_idx, double safe, 
   r[13] = idx, r[14] = next_idx, r[15] = 0;
 }
 
+// the blend of the initial velocity with the bodies' u_def before the time loop (main.cpp:6566-6575): one CTA of 256 threads
+// handles 2 blocks (128 cells x (u, v)) per pass, block-strided; explicit round-to-nearest in the reference's expression order
+__global__ void __launch_bounds__(256)
+amr_udef_blend_kernel(double *__restrict__ vel, const double *__restrict__ tmpv, const double *__restrict__ chi, int64_t nb) {
+  const int64_t n = nb * 128;
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) {
+    const double x = chi[i >> 1];
+    vel[i] = __dadd_rn(__dmul_rn(vel[i], __dsub_rn(1.0, x)), __dmul_rn(tmpv[i], x));
+  }
+}
+
 // per-call device scratch, grown as needed (freed with the shapes)
 static int og_grow(void **p, size_t *cap, size_t bytes) {
   if (bytes <= *cap) return CUP2D_OK;
@@ -672,6 +684,19 @@ int cup2d_amr_shape_get(cup2d_amr *a, int shape, int32_t *ids, double *chi, doub
     CUP2D_CUDA(cudaStreamSynchronize(a->stream));
   }
   return sh.nob;
+}
+
+int cup2d_amr_udef_blend(cup2d_amr *a) {
+  if (!a) {
+    set_error("null cup2d_amr handle");
+    return CUP2D_EINVAL;
+  }
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  if (a->nb == 0) return CUP2D_OK;
+  const int grid = (int)std::min<int64_t>((a->nb + 1) / 2, AMR_GRID_SMS * 8);
+  amr_udef_blend_kernel<<<grid, 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_TMPV], a->f[CUP2D_CHI], a->nb);
+  CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
 }
 
 } // extern "C"

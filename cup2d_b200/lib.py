@@ -32,7 +32,7 @@ SYMBOLS = [
     "cup2d_amr_pressure_rhs_fast", "cup2d_amr_pressure_gradient_fast", "cup2d_amr_laplacian_fast", "cup2d_amr_set_fast",
     "cup2d_amr_adapt_mesh", "cup2d_amr_regrid", "cup2d_amr_ongrid", "cup2d_amr_shape_get",
     "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times", "cup2d_amr_shape_set_dist", "cup2d_amr_collide",
-    "cup2d_amr_surface", "cup2d_amr_surface_get", "cup2d_amr_forces",
+    "cup2d_amr_surface", "cup2d_amr_surface_get", "cup2d_amr_forces", "cup2d_amr_udef_blend",
 ]
 
 
@@ -159,6 +159,7 @@ def load_library():
     lib.cup2d_amr_shape_integrals.argtypes = [P, I, D, D, D, D, C.POINTER(D)]
     lib.cup2d_amr_penalize.argtypes = [P, I, D, D, D, D, D, D, D]
     lib.cup2d_amr_udef_assemble.argtypes = [P]
+    lib.cup2d_amr_udef_blend.argtypes = [P]
     lib.cup2d_amr_adapt_tags.argtypes = [P, D, I, C.POINTER(D)]
     lib.cup2d_amr_set_ranks.argtypes = [P, I, I, C.POINTER(C.c_int64)]
     lib.cup2d_amr_dump.argtypes = [P, D, C.c_char_p]

@@ -360,6 +360,9 @@ int cup2d_amr_shape_integrals(cup2d_amr *a, int shape, double lambda, double dt,
 int cup2d_amr_penalize(cup2d_amr *a, int shape, double lambda, double dt, double cx, double cy, double us, double vs,
                        double omega);
 int cup2d_amr_udef_assemble(cup2d_amr *a);
+/* main.cpp:6566-6575, once before the time loop: vel = vel (1 - chi) + tmpV chi on every cell of the context's blocks (tmpV as
+ * cup2d_amr_udef_assemble leaves it).  Bit-identical to the reference. */
+int cup2d_amr_udef_blend(cup2d_amr *a);
 
 /* ongrid() on a multi-level mesh (main.cpp:3991-4630; csrc/amr_ongrid.cu): the rasterisation of every body's midline into the
  * chi and tmp fields and into the shape's obstacle blocks, on the device.  The midline kinematics (main.cpp:4029-4207), the
