@@ -208,6 +208,27 @@ class AmrSimulation:
                                          C.byref(err)))
         return dto.value, it.value, err.value
 
+    def step_enqueue(self, cfl=0.5, dt=0.0, tol_abs=0.0, tol_rel=0.0, max_restarts=0, max_iter=1000):
+        """step() without host synchronisation (cup2d_amr_step_enqueue): dt <= 0 runs the dt rule on the device; read the
+        outcome with step_result()"""
+        _l.check(self.lib.cup2d_amr_step_enqueue(self._h, float(cfl), float(dt), float(tol_abs), float(tol_rel), int(max_restarts),
+                                                 int(max_iter)))
+
+    def pressure_enqueue(self, dt, tol_abs=0.0, tol_rel=0.0, max_restarts=0, max_iter=1000):
+        """the pressure section alone (poisson_rhs with u_def = tmpV, solve, pressure_correct), enqueued: after udef_assemble"""
+        _l.check(self.lib.cup2d_amr_pressure_enqueue(self._h, float(dt), float(tol_abs), float(tol_rel), int(max_restarts),
+                                                     int(max_iter)))
+
+    def step_result(self):
+        """waits for the last enqueued step / pressure section: (dt, Krylov iterations, residual)"""
+        dto, it, err = C.c_double(), C.c_int(), C.c_double()
+        _l.check(self.lib.cup2d_amr_step_result(self._h, C.byref(dto), C.byref(it), C.byref(err)))
+        return dto.value, it.value, err.value
+
+    def set_graph(self, on=True):
+        """on: from the second enqueue of a form, replay it as one CUDA graph (default); off: launch the kernels directly"""
+        _l.check(self.lib.cup2d_amr_set_graph(self._h, int(on)))
+
     def set_ranks(self, rank, rank_begin, dist=None):
         """several GPUs, first form: this context (whole mesh, operators replicated) solves its Poisson problem together with
         the other ranks, each owning the block range rank_begin[r]..rank_begin[r+1]; `dist` carries the peer blobs"""

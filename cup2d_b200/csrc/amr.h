@@ -49,8 +49,30 @@ struct FluxBuf { // where the face fluxes of the irregular blocks live: per irre
 struct CoarseFace { // one coarse-fine face seen from the coarse side
   int coarse, face, fine[2]; // fine[half] = the fine block abutting that half of the face (-1: absent)
 };
+// A scalar argument of a multi-level kernel (dt, a pressure mean): by value, as the blocking calls pass it, or read from
+// device memory that an earlier kernel of the same enqueued step wrote (cup2d_amr_step_enqueue).  A kernel resolves it once,
+// then computes exactly what it computes from a double; ByValue is passed and read like one.
+struct ByValue {
+  double v;
+  __device__ __forceinline__ double get() const { return v; }
+};
+struct OnDevice {
+  const double *p;
+  __device__ __forceinline__ double get() const { return *p; }
+};
+// launch(ByValue{v}) or, with a device address, launch(OnDevice{p})
+template <class F> inline int with_scalar(double v, const double *p, F &&launch) {
+  return p ? launch(OnDevice{p}) : launch(ByValue{v});
+}
+// the record an enqueued step keeps on the device: its dt, the two h^2-weighted pressure means
+enum { AMR_REC_DT = 0, AMR_REC_MEAN0 = 1, AMR_REC_MEAN1 = 2, AMR_REC_N = 4 };
 
 } // namespace cup2d
+
+// the dt-dependent operators with dt by value (ddt = nullptr) or from the device record of an enqueued step (csrc/amr_fast.cu)
+int amr_advect_rhs_fast(cup2d_amr *a, double dt, const double *ddt);
+int amr_pressure_rhs_fast(cup2d_amr *a, double dt, int with_laplacian, const double *ddt);
+int amr_pressure_gradient_fast(cup2d_amr *a, double dt, const double *ddt);
 
 // the plan's block list, [n][3] (level, i, j), and its level-0 blocks per direction
 const std::vector<int> &amr_plan_level_ij(const cup2d_amr_plan *p, int *bpdx, int *bpdy);
@@ -133,6 +155,15 @@ struct cup2d_amr {
   std::vector<Surface> surf;
   double *d_fo_part = nullptr;      // [obstacle blocks][19] per-block accumulators, then [nshapes][19] sums
   size_t fo_part_cap = 0;
+  // enqueued steps (cup2d_amr_step_enqueue / _pressure_enqueue, csrc/amr_ops.cu): the device record (AMR_REC_*), the events
+  // that join the Poisson context's stream to this one, one executable graph per argument set (cudaGraphExec_t / cudaGraph_t)
+  double *d_rec = nullptr;
+  void *ev_fork = nullptr, *ev_join = nullptr;
+  struct StepGraph { std::vector<unsigned long long> key; void *exec = nullptr, *graph = nullptr; };
+  std::vector<StepGraph> graphs;
+  bool use_graph = true;            // cup2d_amr_set_graph; stays with the handle across a regrid
+  unsigned warmed = 0;              // bit (2 fast + pressure-only): that form has run directly once on this mesh
+  bool step_pending = false;        // an enqueued step / pressure section whose result has not been read
   void free_shapes() {
     for (auto &sh : shapes) {
       cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);

@@ -40,10 +40,12 @@ constexpr int AF_RS = 9;                   // partial-result row stride
 constexpr int AF_BLK = 2 * AF_PLANE + 2 * 8 * AF_RS; // doubles of shared memory per block: su, sv, Ru, Rv
 constexpr int AF_SMEM = AF_WARPS * AF_BPW * AF_BLK * 8; // 72 192 B per CTA -> 3 CTAs/SM
 
+template <class DT>
 __global__ void __launch_bounds__(AF_NT)
 amr_advect_fast_kernel(const double *__restrict__ vel, double *__restrict__ out, const int4 *__restrict__ nbr4,
                        const int *__restrict__ irr_of, const GhostDev gt, const double *__restrict__ hb,
-                       const FluxBuf faceflux, int nb, double nu, double dt) {
+                       const FluxBuf faceflux, int nb, double nu, DT dt_arg) {
+  const double dt = dt_arg.get();
   extern __shared__ __align__(16) double af_smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int q = lane >> 3, r = lane & 7;
@@ -187,10 +189,12 @@ __device__ __forceinline__ void face_pos(int f, int t, int &pi, int &pg) { // in
 }
 
 // tmp = pressure_rhs(vel, u_def, chi) (main.cpp:6105-6139) + the face fluxes of main.cpp:6152-6205
+template <class DT>
 __global__ void __launch_bounds__(A1_NT)
 amr_div_fast_kernel(const double *__restrict__ vel, const double *__restrict__ udef, const double *__restrict__ chi,
                     double *__restrict__ tmp, const int4 *__restrict__ nbr4, const int *__restrict__ irr_of, const GhostDev gt,
-                    const double *__restrict__ hb, const FluxBuf faceflux, int nb, double dt) {
+                    const double *__restrict__ hb, const FluxBuf faceflux, int nb, DT dt_arg) {
+  const double dt = dt_arg.get();
   __shared__ double s_lab[A1_WARPS * 4 * 4 * A1_PLANE];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane >> 3, r = lane & 7;
   const int b0 = (blockIdx.x * A1_WARPS + warp) * 4;
@@ -230,11 +234,12 @@ amr_div_fast_kernel(const double *__restrict__ vel, const double *__restrict__ u
 }
 
 // MODE 0: tmp -= lap(p) (main.cpp:6209-6230) + face fluxes (6243-6283);  MODE 1: tmpV = pressureCorrectionKernel(p) (6021-6043)
-template <int MODE>
+template <int MODE, class DT>
 __global__ void __launch_bounds__(A1_NT)
 amr_scalar_fast_kernel(const double *__restrict__ p, double *__restrict__ out, const int4 *__restrict__ nbr4,
                        const int *__restrict__ irr_of, const GhostDev gt, const double *__restrict__ hb,
-                       const FluxBuf faceflux, int nb, double dt) {
+                       const FluxBuf faceflux, int nb, DT dt_arg) {
+  const double dt = dt_arg.get();
   __shared__ double s_lab[A1_WARPS * 4 * A1_PLANE];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane >> 3, r = lane & 7;
   const int b0 = (blockIdx.x * A1_WARPS + warp) * 4;
@@ -313,7 +318,8 @@ template <int DIM> static int fluxcorr_faces(cup2d_amr *a, double *result) {
 
 static int fast_constants() {
   CUP2D_CUDA(cudaMemcpyToSymbol(cW, hW, sizeof hW));
-  CUP2D_CUDA(cudaFuncSetAttribute(amr_advect_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM));
+  CUP2D_CUDA(cudaFuncSetAttribute(amr_advect_fast_kernel<ByValue>, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM));
+  CUP2D_CUDA(cudaFuncSetAttribute(amr_advect_fast_kernel<OnDevice>, cudaFuncAttributeMaxDynamicSharedMemorySize, AF_SMEM));
   return CUP2D_OK;
 }
 
@@ -365,6 +371,58 @@ static int fast_setup(cup2d_amr *a) {
 } // namespace cup2d
 
 int amr_fast_tables(cup2d_amr *a) { return cup2d::fast_setup(a); }
+
+int amr_advect_rhs_fast(cup2d_amr *a, double dt, const double *ddt) {
+  using namespace cup2d;
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  int rc = fast_setup(a);
+  if (rc) return rc;
+  if ((rc = amr_dist_refresh(a, CUP2D_VEL))) return rc;
+  const int per_cta = AF_WARPS * AF_BPW;
+  const int grid = (int)((a->nb + per_cta - 1) / per_cta);
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_advect_fast_kernel<<<grid, AF_NT, AF_SMEM, a->stream>>>(
+        a->f[CUP2D_VEL], a->f[CUP2D_TMPV], reinterpret_cast<const int4 *>(a->d_nbr4), a->d_irr_of, a->gt[0], a->d_h,
+        flux_buf<2>(a), (int)a->nb, a->nu, d);
+    return 0;
+  });
+  CUP2D_CUDA(cudaGetLastError());
+  return fluxcorr_faces<2>(a, a->f[CUP2D_TMPV]);
+}
+
+int amr_pressure_rhs_fast(cup2d_amr *a, double dt, int with_laplacian, const double *ddt) {
+  using namespace cup2d;
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  int rc = fast_setup(a);
+  if (rc) return rc;
+  if ((rc = amr_dist_refresh(a, CUP2D_VEL)) || (rc = amr_dist_refresh(a, CUP2D_TMPV))) return rc;
+  const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
+  const int4 *nbr4 = reinterpret_cast<const int4 *>(a->d_nbr4);
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_div_fast_kernel<<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_TMPV], a->f[CUP2D_CHI], a->f[CUP2D_TMP], nbr4,
+                                                       a->d_irr_of, a->gt[1], a->d_h, flux_buf<1>(a), (int)a->nb, d);
+    return 0;
+  });
+  CUP2D_CUDA(cudaGetLastError());
+  if ((rc = fluxcorr_faces<1>(a, a->f[CUP2D_TMP])) || !with_laplacian) return rc;
+  return cup2d_amr_laplacian_fast(a, dt);
+}
+
+int amr_pressure_gradient_fast(cup2d_amr *a, double dt, const double *ddt) {
+  using namespace cup2d;
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  int rc = fast_setup(a);
+  if (rc) return rc;
+  if ((rc = amr_dist_refresh(a, CUP2D_PRES))) return rc;
+  const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_scalar_fast_kernel<1><<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_PRES], a->f[CUP2D_TMPV], reinterpret_cast<const int4 *>(a->d_nbr4),
+                                                             a->d_irr_of, a->gt[2], a->d_h, flux_buf<1>(a), (int)a->nb, d);
+    return 0;
+  });
+  CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
+}
 
 // Tables of a DISTRIBUTED context: the plan knows the whole mesh; this rank keeps what concerns its blocks [b0, b1) and
 // names every block by its local slot (own blocks first, then the halo slots of the field arrays): slot_of[global block] or -1.
@@ -472,17 +530,7 @@ int cup2d_amr_advect_diffuse_rhs_fast(cup2d_amr *a, double dt) {
     set_error("null cup2d_amr handle");
     return CUP2D_EINVAL;
   }
-  CUP2D_CUDA(cudaSetDevice(a->device));
-  int rc = fast_setup(a);
-  if (rc) return rc;
-  if ((rc = amr_dist_refresh(a, CUP2D_VEL))) return rc;
-  const int per_cta = AF_WARPS * AF_BPW;
-  const int grid = (int)((a->nb + per_cta - 1) / per_cta);
-  amr_advect_fast_kernel<<<grid, AF_NT, AF_SMEM, a->stream>>>(
-      a->f[CUP2D_VEL], a->f[CUP2D_TMPV], reinterpret_cast<const int4 *>(a->d_nbr4), a->d_irr_of, a->gt[0], a->d_h,
-      flux_buf<2>(a), (int)a->nb, a->nu, dt);
-  CUP2D_CUDA(cudaGetLastError());
-  return fluxcorr_faces<2>(a, a->f[CUP2D_TMPV]);
+  return amr_advect_rhs_fast(a, dt, nullptr);
 }
 
 /* same results as cup2d_amr_pressure_rhs / cup2d_amr_pressure_gradient through per-block +-1 labs in shared memory */
@@ -491,17 +539,7 @@ int cup2d_amr_pressure_rhs_fast(cup2d_amr *a, double dt, int with_laplacian) {
     set_error("null cup2d_amr handle");
     return CUP2D_EINVAL;
   }
-  CUP2D_CUDA(cudaSetDevice(a->device));
-  int rc = fast_setup(a);
-  if (rc) return rc;
-  if ((rc = amr_dist_refresh(a, CUP2D_VEL)) || (rc = amr_dist_refresh(a, CUP2D_TMPV))) return rc;
-  const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
-  const int4 *nbr4 = reinterpret_cast<const int4 *>(a->d_nbr4);
-  amr_div_fast_kernel<<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_TMPV], a->f[CUP2D_CHI], a->f[CUP2D_TMP], nbr4,
-                                                     a->d_irr_of, a->gt[1], a->d_h, flux_buf<1>(a), (int)a->nb, dt);
-  CUP2D_CUDA(cudaGetLastError());
-  if ((rc = fluxcorr_faces<1>(a, a->f[CUP2D_TMP])) || !with_laplacian) return rc;
-  return cup2d_amr_laplacian_fast(a, dt);
+  return amr_pressure_rhs_fast(a, dt, with_laplacian, nullptr);
 }
 
 /* tmp -= lap(pold), flux-corrected (main.cpp:7022-7027) */
@@ -516,7 +554,7 @@ int cup2d_amr_laplacian_fast(cup2d_amr *a, double dt) {
   if ((rc = amr_dist_refresh(a, CUP2D_POLD))) return rc;
   const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
   amr_scalar_fast_kernel<0><<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_POLD], a->f[CUP2D_TMP], reinterpret_cast<const int4 *>(a->d_nbr4),
-                                                           a->d_irr_of, a->gt[2], a->d_h, flux_buf<1>(a), (int)a->nb, dt);
+                                                           a->d_irr_of, a->gt[2], a->d_h, flux_buf<1>(a), (int)a->nb, ByValue{dt});
   CUP2D_CUDA(cudaGetLastError());
   return fluxcorr_faces<1>(a, a->f[CUP2D_TMP]);
 }
@@ -537,15 +575,7 @@ int cup2d_amr_pressure_gradient_fast(cup2d_amr *a, double dt) {
     set_error("null cup2d_amr handle");
     return CUP2D_EINVAL;
   }
-  CUP2D_CUDA(cudaSetDevice(a->device));
-  int rc = fast_setup(a);
-  if (rc) return rc;
-  if ((rc = amr_dist_refresh(a, CUP2D_PRES))) return rc;
-  const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
-  amr_scalar_fast_kernel<1><<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_PRES], a->f[CUP2D_TMPV], reinterpret_cast<const int4 *>(a->d_nbr4),
-                                                           a->d_irr_of, a->gt[2], a->d_h, flux_buf<1>(a), (int)a->nb, dt);
-  CUP2D_CUDA(cudaGetLastError());
-  return CUP2D_OK;
+  return amr_pressure_gradient_fast(a, dt, nullptr);
 }
 
 } // extern "C"

@@ -16,7 +16,9 @@
 //      corrected (property 4).
 #include "sim.h"
 #include <algorithm>
+#include <cmath>
 #include <map>
+#include <string>
 #include <vector>
 
 #include "amr.h"
@@ -83,8 +85,10 @@ __device__ __forceinline__ double L2(const double *lab, int64_t k, int ix, int i
   return lab[(k * 10 + (iy + 1)) * 10 + (ix + 1)];
 }
 
+template <class DT>
 __global__ void amr_advect_kernel(const double *__restrict__ lab, double *__restrict__ out, const double *__restrict__ hb,
-                                  int64_t ncells, double nu, double dt) {
+                                  int64_t ncells, double nu, DT dt_arg) {
+  const double dt = dt_arg.get();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ncells; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t k = i >> 6;
     const int ix = (int)(i & 7), iy = (int)((i >> 3) & 7);
@@ -101,9 +105,11 @@ __global__ void amr_advect_kernel(const double *__restrict__ lab, double *__rest
   }
 }
 
+template <class DT>
 __global__ void amr_div_kernel(const double *__restrict__ labv, const double *__restrict__ labu,
                                const double *__restrict__ chi, double *__restrict__ tmp, const double *__restrict__ hb,
-                               int64_t ncells, double dt) {
+                               int64_t ncells, DT dt_arg) {
+  const double dt = dt_arg.get();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ncells; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t k = i >> 6;
     const int ix = (int)(i & 7), iy = (int)((i >> 3) & 7);
@@ -123,8 +129,10 @@ __global__ void amr_lap_kernel(const double *__restrict__ labp, double *__restri
   }
 }
 
+template <class DT>
 __global__ void amr_gradp_kernel(const double *__restrict__ labp, double *__restrict__ tmpv, const double *__restrict__ hb,
-                                 int64_t ncells, double dt) {
+                                 int64_t ncells, DT dt_arg) {
+  const double dt = dt_arg.get();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ncells; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t k = i >> 6;
     const int ix = (int)(i & 7), iy = (int)((i >> 3) & 7);
@@ -196,8 +204,10 @@ __global__ void amr_block_wsum_kernel(const double *__restrict__ p, const double
   }
 }
 // p[i] = (src ? src[i] : p[i]) + (add ? add[i] : 0) - shift
+template <class S>
 __global__ void amr_shift_kernel(double *__restrict__ p, const double *__restrict__ src, const double *__restrict__ add,
-                                 int64_t n, double shift) {
+                                 int64_t n, S shift_arg) {
+  const double shift = shift_arg.get();
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     double v = src ? src[i] : p[i];
     if (add) v += add[i] - shift; else v += -shift;
@@ -230,13 +240,14 @@ __device__ __forceinline__ double face_flux(const double *labA, const double *la
 }
 
 // one thread per (coarse face, position t, comp): coarse cell += [own flux + (fine a + fine b)], twice where the reference does
-template <int MODE>
+template <int MODE, class DT>
 __global__ void amr_fluxcorr_kernel(const CoarseFace *__restrict__ cf, int ncf, const double *labA, const double *labB,
                                     const double *chi, const double *hb, double *__restrict__ result, double nu,
-                                    double dt) {
+                                    DT dt_arg) {
   constexpr int DIM = MODE == 0 ? 2 : 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= ncf * 8 * DIM) return;
+  const double dt = dt_arg.get();
   const int comp = i % DIM, t = (i / DIM) % 8;
   const CoarseFace f = cf[i / (8 * DIM)];
   double acc = face_flux<MODE>(labA, labB, chi, hb, f.coarse, f.face, t, comp, nu, dt);
@@ -317,13 +328,16 @@ static int gather(cup2d_amr *a, int which, const double *field, double *&lab) {
 }
 
 template <int MODE>
-static int fluxcorr(cup2d_amr *a, const double *labA, const double *labB, double *result, double dt) {
+static int fluxcorr(cup2d_amr *a, const double *labA, const double *labB, double *result, double dt, const double *ddt = nullptr) {
   constexpr int DIM = MODE == 0 ? 2 : 1;
   for (int dir = 0; dir < 2; dir++) { // x faces, then y faces (fillcases order)
     const int n = a->ncf[dir] * 8 * DIM;
     if (n == 0) continue;
-    amr_fluxcorr_kernel<MODE><<<(n + 127) / 128, 128, 0, a->stream>>>(a->d_cf[dir], a->ncf[dir], labA, labB, a->f[CUP2D_CHI],
-                                                                      a->d_h, result, a->nu, dt);
+    with_scalar(dt, ddt, [&](auto d) {
+      amr_fluxcorr_kernel<MODE><<<(n + 127) / 128, 128, 0, a->stream>>>(a->d_cf[dir], a->ncf[dir], labA, labB, a->f[CUP2D_CHI],
+                                                                        a->d_h, result, a->nu, d);
+      return 0;
+    });
   }
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;
@@ -430,8 +444,15 @@ void cup2d_amr_destroy(cup2d_amr *a) {
     cudaFree(g.grow); cudaFree(g.rowptr); cudaFree(g.dst); cudaFree(g.sb); cudaFree(g.sc); cudaFree(g.w);
   }
 #ifndef CUP2D_AMR_EMU
+  for (auto &g : a->graphs) {
+    if (g.exec) cudaGraphExecDestroy((cudaGraphExec_t)g.exec);
+    if (g.graph) cudaGraphDestroy((cudaGraph_t)g.graph);
+  }
+  if (a->ev_fork) cudaEventDestroy((cudaEvent_t)a->ev_fork);
+  if (a->ev_join) cudaEventDestroy((cudaEvent_t)a->ev_join);
   if (a->poisson) cup2d_destroy(a->poisson);
 #endif
+  cudaFree(a->d_rec);
   if (a->stream && !a->dist) cudaStreamDestroy(a->stream);
   if (a->plan) cup2d_amr_plan_destroy(a->plan);
   delete a;
@@ -455,30 +476,34 @@ int cup2d_amr_field_download(cup2d_amr *a, int field, double *host) {
   return CUP2D_OK;
 }
 
-/* tmpV = KernelAdvectDiffuse(vel), flux-corrected (main.cpp:6611-6617) */
-int cup2d_amr_advect_diffuse_rhs(cup2d_amr *a, double dt) {
-  CHECK_AMR(a);
-  if (a->fast) return cup2d_amr_advect_diffuse_rhs_fast(a, dt);
+} // extern "C"
+
+// the dt-dependent operators, dt by value (ddt = nullptr: the blocking calls) or from the device record of an enqueued step
+static int advect_rhs(cup2d_amr *a, double dt, const double *ddt) {
+  if (a->fast) return amr_advect_rhs_fast(a, dt, ddt);
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc = gather(a, 0, a->f[CUP2D_VEL], a->lab[0]);
   if (rc) return rc;
-  amr_advect_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[0], a->f[CUP2D_TMPV], a->d_h, a->nb * 64, a->nu, dt);
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_advect_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[0], a->f[CUP2D_TMPV], a->d_h, a->nb * 64, a->nu, d);
+    return 0;
+  });
   CUP2D_CUDA(cudaGetLastError());
-  return fluxcorr<0>(a, a->lab[0], nullptr, a->f[CUP2D_TMPV], dt);
+  return fluxcorr<0>(a, a->lab[0], nullptr, a->f[CUP2D_TMPV], dt, ddt);
 }
 
-/* tmp = pressure_rhs(vel, u_def = tmpV, chi), flux-corrected (main.cpp:7007-7013); with_laplacian: then
- * tmp -= lap(pold), flux-corrected (main.cpp:7022-7027) */
-int cup2d_amr_pressure_rhs(cup2d_amr *a, double dt, int with_laplacian) {
-  CHECK_AMR(a);
-  if (a->fast) return cup2d_amr_pressure_rhs_fast(a, dt, with_laplacian);
+static int pressure_rhs(cup2d_amr *a, double dt, int with_laplacian, const double *ddt) {
+  if (a->fast) return amr_pressure_rhs_fast(a, dt, with_laplacian, ddt);
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc = gather(a, 1, a->f[CUP2D_VEL], a->lab[1]);
   if (rc || (rc = gather(a, 1, a->f[CUP2D_TMPV], a->lab_udef))) return rc;
-  amr_div_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[1], a->lab_udef, a->f[CUP2D_CHI], a->f[CUP2D_TMP], a->d_h,
-                                                             a->nb * 64, dt);
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_div_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[1], a->lab_udef, a->f[CUP2D_CHI], a->f[CUP2D_TMP], a->d_h,
+                                                               a->nb * 64, d);
+    return 0;
+  });
   CUP2D_CUDA(cudaGetLastError());
-  if ((rc = fluxcorr<1>(a, a->lab[1], a->lab_udef, a->f[CUP2D_TMP], dt))) return rc;
+  if ((rc = fluxcorr<1>(a, a->lab[1], a->lab_udef, a->f[CUP2D_TMP], dt, ddt))) return rc;
   if (!with_laplacian) return CUP2D_OK;
   if ((rc = gather(a, 2, a->f[CUP2D_POLD], a->lab[2]))) return rc;
   amr_lap_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[2], a->f[CUP2D_TMP], a->nb * 64);
@@ -486,16 +511,38 @@ int cup2d_amr_pressure_rhs(cup2d_amr *a, double dt, int with_laplacian) {
   return fluxcorr<2>(a, a->lab[2], nullptr, a->f[CUP2D_TMP], dt);
 }
 
-/* tmpV = pressureCorrectionKernel(pres) (main.cpp:7174-7179; not flux-corrected in the reference either) */
-int cup2d_amr_pressure_gradient(cup2d_amr *a, double dt) {
-  CHECK_AMR(a);
-  if (a->fast) return cup2d_amr_pressure_gradient_fast(a, dt);
+static int pressure_gradient(cup2d_amr *a, double dt, const double *ddt) {
+  if (a->fast) return amr_pressure_gradient_fast(a, dt, ddt);
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc = gather(a, 2, a->f[CUP2D_PRES], a->lab[2]);
   if (rc) return rc;
-  amr_gradp_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[2], a->f[CUP2D_TMPV], a->d_h, a->nb * 64, dt);
+  with_scalar(dt, ddt, [&](auto d) {
+    amr_gradp_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[2], a->f[CUP2D_TMPV], a->d_h, a->nb * 64, d);
+    return 0;
+  });
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;
+}
+
+extern "C" {
+
+/* tmpV = KernelAdvectDiffuse(vel), flux-corrected (main.cpp:6611-6617) */
+int cup2d_amr_advect_diffuse_rhs(cup2d_amr *a, double dt) {
+  CHECK_AMR(a);
+  return advect_rhs(a, dt, nullptr);
+}
+
+/* tmp = pressure_rhs(vel, u_def = tmpV, chi), flux-corrected (main.cpp:7007-7013); with_laplacian: then
+ * tmp -= lap(pold), flux-corrected (main.cpp:7022-7027) */
+int cup2d_amr_pressure_rhs(cup2d_amr *a, double dt, int with_laplacian) {
+  CHECK_AMR(a);
+  return pressure_rhs(a, dt, with_laplacian, nullptr);
+}
+
+/* tmpV = pressureCorrectionKernel(pres) (main.cpp:7174-7179; not flux-corrected in the reference either) */
+int cup2d_amr_pressure_gradient(cup2d_amr *a, double dt) {
+  CHECK_AMR(a);
+  return pressure_gradient(a, dt, nullptr);
 }
 
 static int block_partials(cup2d_amr *a, int n_per_block) {
@@ -581,14 +628,14 @@ int cup2d_amr_compute_dt(cup2d_amr *a, double cfl, double *umax_out, double *dt_
   return CUP2D_OK;
 }
 
-/* main.cpp:6607-6642: vold = vel; vel = vold + 0.5 K(vel)/h^2; vel = vold + K(vel)/h^2 (K flux-corrected) */
-int cup2d_amr_advect_diffuse_rk2(cup2d_amr *a, double dt) {
-  CHECK_AMR(a);
+} // extern "C"
+
+static int rk2(cup2d_amr *a, double dt, const double *ddt) {
   CUP2D_CUDA(cudaSetDevice(a->device));
   const int64_t n = a->nb * 128;
   CUP2D_CUDA(cudaMemcpyAsync(a->f[CUP2D_VOLD], a->f[CUP2D_VEL], n * sizeof(double), cudaMemcpyDeviceToDevice, a->stream));
   for (int stage = 0; stage < 2; stage++) {
-    int rc = cup2d_amr_advect_diffuse_rhs(a, dt);
+    int rc = advect_rhs(a, dt, ddt);
     if (rc) return rc;
     amr_axpy_h2_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_VOLD], a->f[CUP2D_TMPV], a->d_h, n,
                                                           stage == 0 ? 0.5 : 1.0);
@@ -597,11 +644,9 @@ int cup2d_amr_advect_diffuse_rk2(cup2d_amr *a, double dt) {
   return CUP2D_OK;
 }
 
-/* main.cpp:7007-7027 as one call: tmp = pressure_rhs(vel, u_def = tmpV, chi); pold = pres; pres = 0; tmp -= lap(pold) */
-int cup2d_amr_poisson_rhs(cup2d_amr *a, double dt) {
-  CHECK_AMR(a);
+static int poisson_rhs(cup2d_amr *a, double dt, const double *ddt) {
   CUP2D_CUDA(cudaSetDevice(a->device));
-  int rc = cup2d_amr_pressure_rhs(a, dt, 0);
+  int rc = pressure_rhs(a, dt, 0, ddt);
   if (rc) return rc;
   const size_t bytes = (size_t)a->nb * 64 * sizeof(double);
   CUP2D_CUDA(cudaMemcpyAsync(a->f[CUP2D_POLD], a->f[CUP2D_PRES], bytes, cudaMemcpyDeviceToDevice, a->stream));
@@ -611,6 +656,20 @@ int cup2d_amr_poisson_rhs(cup2d_amr *a, double dt) {
   amr_lap_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[2], a->f[CUP2D_TMP], a->nb * 64);
   CUP2D_CUDA(cudaGetLastError());
   return fluxcorr<2>(a, a->lab[2], nullptr, a->f[CUP2D_TMP], dt);
+}
+
+extern "C" {
+
+/* main.cpp:6607-6642: vold = vel; vel = vold + 0.5 K(vel)/h^2; vel = vold + K(vel)/h^2 (K flux-corrected) */
+int cup2d_amr_advect_diffuse_rk2(cup2d_amr *a, double dt) {
+  CHECK_AMR(a);
+  return rk2(a, dt, nullptr);
+}
+
+/* main.cpp:7007-7027 as one call: tmp = pressure_rhs(vel, u_def = tmpV, chi); pold = pres; pres = 0; tmp -= lap(pold) */
+int cup2d_amr_poisson_rhs(cup2d_amr *a, double dt) {
+  CHECK_AMR(a);
+  return poisson_rhs(a, dt, nullptr);
 }
 
 static int weighted_mean(cup2d_amr *a, const double *p, double *mean) {
@@ -634,9 +693,9 @@ int cup2d_amr_pressure_correct(cup2d_amr *a, double dt) {
   double avg = 0;
   int rc = weighted_mean(a, a->f[CUP2D_PRES], &avg);
   if (rc) return rc;
-  amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, nullptr, n, avg);
+  amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, nullptr, n, ByValue{avg});
   if ((rc = weighted_mean(a, a->f[CUP2D_PRES], &avg))) return rc;
-  amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, a->f[CUP2D_POLD], n, avg);
+  amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, a->f[CUP2D_POLD], n, ByValue{avg});
   CUP2D_CUDA(cudaGetLastError());
   if ((rc = cup2d_amr_pressure_gradient(a, dt))) return rc;
   amr_axpy_h2_kernel<<<grid_for(2 * n), 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_VEL], a->f[CUP2D_TMPV], a->d_h, 2 * n, 1.0);
@@ -841,22 +900,25 @@ static int poisson_solve_distributed(cup2d_amr *a, double tol_abs, double tol_re
 
 /* the Poisson solve of the step: b = tmp, x0 = pres -> pres, on the general-rows solver (csrc/poisson.cu) with the
  * rows of cup2d_amr_plan_poisson; same stopping parameters as cup2d_poisson_solve */
+// the general-rows Poisson context over the blocks of the mesh, created on first use
+static int ensure_poisson(cup2d_amr *a) {
+  if (a->poisson) return CUP2D_OK;
+  int64_t nnz = 0;
+  const int64_t nr = cup2d_amr_plan_poisson(a->plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
+  if (nr < 0) return (int)nr;
+  std::vector<int32_t> nbr(4 * a->nb), rows(std::max<int64_t>(nr, 1)), rowptr(nr + 1), col(std::max<int64_t>(nnz, 1));
+  std::vector<double> val(std::max<int64_t>(nnz, 1));
+  cup2d_amr_plan_poisson(a->plan, nbr.data(), &nnz, rows.data(), rowptr.data(), col.data(), val.data());
+  return cup2d_poisson_create_general(a->nb, nbr.data(), nr, rows.data(), rowptr.data(), col.data(), val.data(), a->device,
+                                      &a->poisson);
+}
+
 int cup2d_amr_poisson_solve(cup2d_amr *a, double tol_abs, double tol_rel, int max_restarts, int max_iter, int *iters,
                             double *err) {
   CHECK_AMR(a);
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc;
-  if (!a->poisson) {
-    int64_t nnz = 0;
-    const int64_t nr = cup2d_amr_plan_poisson(a->plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
-    if (nr < 0) return (int)nr;
-    std::vector<int32_t> nbr(4 * a->nb), rows(std::max<int64_t>(nr, 1)), rowptr(nr + 1), col(std::max<int64_t>(nnz, 1));
-    std::vector<double> val(std::max<int64_t>(nnz, 1));
-    cup2d_amr_plan_poisson(a->plan, nbr.data(), &nnz, rows.data(), rowptr.data(), col.data(), val.data());
-    if ((rc = cup2d_poisson_create_general(a->nb, nbr.data(), nr, rows.data(), rowptr.data(), col.data(), val.data(), a->device,
-                                           &a->poisson)))
-      return rc;
-  }
+  if ((rc = ensure_poisson(a))) return rc;
   if (a->dist) { // the fields ARE the Poisson context's: b = tmp and x0 = pres are in place, so is the result
     CUP2D_CUDA(cudaSetDevice(a->device));
     return cup2d_poisson_solve(a->poisson, tol_abs, tol_rel, max_restarts, max_iter, iters, err);
@@ -886,6 +948,250 @@ int cup2d_amr_step(cup2d_amr *a, double cfl, double dt_in, double tol_abs, doubl
   if ((rc = cup2d_amr_poisson_solve(a, tol_abs, tol_rel, max_restarts, max_iter, iters, err))) return rc;
   if ((rc = cup2d_amr_pressure_correct(a, dt))) return rc;
   if (dt_out) *dt_out = dt;
+  return CUP2D_OK;
+}
+
+} // extern "C"
+
+// ---- time steps enqueued without host synchronisation (cup2d_amr_step_enqueue / _pressure_enqueue) --------------------
+// The blocking calls above wait on the host for dt (per-block maxima), for the two pressure means (per-block sums) and for
+// the Krylov solve.  Here dt lives in the device record a->d_rec and every dt-dependent kernel reads it from there
+// (OnDevice), the means are reduced on the device into the same record, and the solve is enqueued on the Poisson context's
+// stream, joined to this one by events: nothing in the body depends on a host value that changes from step to step, so it
+// is captured once per argument set into a CUDA graph and replayed with one cudaGraphLaunch.
+namespace cup2d {
+
+constexpr int AMR_RED_NT = 1024; // one CTA reduces the per-block partials of the whole mesh
+
+// dt given by value: written by a kernel ahead of the graph launch, so that the graph does not hold it
+__global__ void amr_set_dt_kernel(double *rec, double dt) { rec[AMR_REC_DT] = dt; }
+
+// the dt rule of cup2d_amr_compute_dt: the largest per-block maximum (a maximum is exact in any order), then main.cpp:6593-6595
+// in the host code's operation order with explicit round-to-nearest operations (no FMA contraction): bitwise the host's dt
+__global__ void __launch_bounds__(AMR_RED_NT) amr_dt_kernel(const double *__restrict__ part, int64_t nb, double h, double nu,
+                                                            double cfl, double *rec) {
+  __shared__ double sm[AMR_RED_NT];
+  double m = 0.0;
+  for (int64_t k = threadIdx.x; k < nb; k += AMR_RED_NT) m = fmax(m, part[k]);
+  sm[threadIdx.x] = m;
+  __syncthreads();
+  for (int s = AMR_RED_NT / 2; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) sm[threadIdx.x] = fmax(sm[threadIdx.x], sm[threadIdx.x + s]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double umax = sm[0];
+    const double dt_diff = __ddiv_rn(__dmul_rn(__dmul_rn(0.25, h), h), __dadd_rn(nu, __dmul_rn(__dmul_rn(0.25, h), umax)));
+    const double dt_adv = __ddiv_rn(h, __dadd_rn(umax, 1e-8));
+    const double c = __dmul_rn(cfl, dt_adv);
+    rec[AMR_REC_DT] = c < dt_diff ? c : dt_diff; // std::min(dt_diff, c)
+  }
+}
+
+// sum(P h^2) / sum(h^2) over the per-block pairs of amr_block_wsum_kernel in a FIXED order, so that a step gives the same bits
+// every time: thread t adds the blocks t, t + NT, t + 2 NT, ... in block order, then the NT partial sums are combined by a
+// binary tree (s[t] += s[t + m] for m = NT/2, ..., 1).  The blocking path adds the blocks in one serial chain on the host;
+// the two orders agree to rounding.
+__global__ void __launch_bounds__(AMR_RED_NT) amr_wmean_kernel(const double *__restrict__ part, int64_t nb, double *mean) {
+  __shared__ double ss[AMR_RED_NT];
+  __shared__ double sw[AMR_RED_NT];
+  const double2 *p2 = reinterpret_cast<const double2 *>(part);
+  double s = 0.0, w = 0.0;
+  for (int64_t k0 = threadIdx.x; k0 < nb; k0 += 4 * AMR_RED_NT) { // four loads in flight per thread, added in block order
+    double2 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int64_t k = k0 + (int64_t)u * AMR_RED_NT;
+      v[u] = k < nb ? p2[k] : double2{0.0, 0.0};
+    }
+#pragma unroll
+    for (int u = 0; u < 4; u++) s += v[u].x, w += v[u].y;
+  }
+  ss[threadIdx.x] = s;
+  sw[threadIdx.x] = w;
+  __syncthreads();
+  for (int m = AMR_RED_NT / 2; m > 0; m >>= 1) {
+    if ((int)threadIdx.x < m) ss[threadIdx.x] += ss[threadIdx.x + m], sw[threadIdx.x] += sw[threadIdx.x + m];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *mean = ss[0] / sw[0];
+}
+
+// dst = the Krylov iterate the solve returns (KrylovState::opt, chosen on the device)
+__global__ void amr_take_x_kernel(double *__restrict__ dst, const double *x0, const double *x1, const double *x2,
+                                  const KrylovState *__restrict__ st, int64_t n) {
+  const int o = st->opt;
+  const double *__restrict__ src = o == 0 ? x0 : o == 1 ? x1 : x2;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) dst[i] = src[i];
+}
+
+} // namespace cup2d
+
+// cup2d_amr_pressure_correct with dt and both means from the device record
+static int pressure_correct_enqueued(cup2d_amr *a) {
+  const int64_t n = a->nb * 64;
+  for (int pass = 0; pass < 2; pass++) { // pres -= mean_h2(pres); then pres += pold - mean_h2(pres)
+    double *mean = a->d_rec + AMR_REC_MEAN0 + pass;
+    amr_block_wsum_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->f[CUP2D_PRES], a->d_h, a->d_part, a->nb);
+    amr_wmean_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, mean);
+    amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, pass ? a->f[CUP2D_POLD] : nullptr, n,
+                                                         OnDevice{mean});
+    CUP2D_CUDA(cudaGetLastError());
+  }
+  int rc = pressure_gradient(a, 0.0, a->d_rec + AMR_REC_DT);
+  if (rc) return rc;
+  amr_axpy_h2_kernel<<<grid_for(2 * n), 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_VEL], a->f[CUP2D_TMPV], a->d_h, 2 * n, 1.0);
+  CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
+}
+
+// the body of an enqueued step (pressure_only = false: cup2d_amr_step without bodies) or pressure section
+static int enqueue_body(cup2d_amr *a, bool pressure_only, bool dev_dt, double cfl, double tol_abs, double tol_rel,
+                        int max_restarts, int max_iter, bool capturing) {
+  const double *ddt = a->d_rec + AMR_REC_DT;
+  const int64_t n = a->nb * 64;
+  int rc;
+  if (!pressure_only) {
+    if (dev_dt) {
+      amr_block_absmax_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->d_part, a->nb);
+      amr_dt_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, a->hmin, a->nu, cfl, a->d_rec);
+      CUP2D_CUDA(cudaGetLastError());
+    }
+    if ((rc = rk2(a, 0.0, ddt))) return rc;
+    CUP2D_CUDA(cudaMemsetAsync(a->f[CUP2D_TMPV], 0, (size_t)n * 2 * sizeof(double), a->stream)); // no bodies: u_def = 0
+  }
+  if ((rc = poisson_rhs(a, 0.0, ddt))) return rc;
+  // b = tmp, x0 = pres into the Poisson context, on its stream after this one's work (the event also pulls that stream
+  // into a capture of this one); the iterate comes back after the solve's last kernel
+  cup2d_sim *ps = a->poisson;
+  CUP2D_CUDA(cudaEventRecord((cudaEvent_t)a->ev_fork, a->stream));
+  CUP2D_CUDA(cudaStreamWaitEvent(ps->stream, (cudaEvent_t)a->ev_fork, 0));
+  CUP2D_CUDA(cudaMemcpyAsync(ps->f[CUP2D_TMP], a->f[CUP2D_TMP], n * sizeof(double), cudaMemcpyDeviceToDevice, ps->stream));
+  CUP2D_CUDA(cudaMemcpyAsync(ps->f[CUP2D_PRES], a->f[CUP2D_PRES], n * sizeof(double), cudaMemcpyDeviceToDevice, ps->stream));
+  if ((rc = poisson_enqueue(ps, tol_abs, tol_rel, max_restarts, max_iter, false, capturing))) return rc;
+  CUP2D_CUDA(cudaEventRecord((cudaEvent_t)a->ev_join, ps->stream));
+  CUP2D_CUDA(cudaStreamWaitEvent(a->stream, (cudaEvent_t)a->ev_join, 0));
+  amr_take_x_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], ps->kx[0], ps->kx[1], ps->kx[2], ps->d_state, n);
+  CUP2D_CUDA(cudaGetLastError());
+  return pressure_correct_enqueued(a);
+}
+
+static int amr_enqueue(cup2d_amr *a, const char *who, bool pressure_only, double cfl, double dt_in, double tol_abs,
+                       double tol_rel, int max_restarts, int max_iter) {
+  CHECK_AMR(a);
+  if (a->dist || !a->rank_begin.empty()) {
+    set_error(std::string(who) + ": contexts on several ranks have the blocking calls only");
+    return CUP2D_ESTATE;
+  }
+  const bool dev_dt = !(dt_in > 0);
+  if (std::isnan(dt_in) || std::isinf(dt_in) || (pressure_only && dev_dt) || (dev_dt && !(cfl > 0 && std::isfinite(cfl))) ||
+      !(tol_abs >= 0) || !(tol_rel >= 0) || max_restarts < 0 || max_iter < 0) {
+    set_error(std::string(who) + ": bad arguments");
+    return CUP2D_EINVAL;
+  }
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  int rc;
+  if ((rc = ensure_poisson(a))) return rc;
+  if (!a->d_rec) CUP2D_CUDA(cudaMalloc(&a->d_rec, AMR_REC_N * sizeof(double)));
+  if (!a->ev_fork) {
+    cudaEvent_t f, j;
+    CUP2D_CUDA(cudaEventCreateWithFlags(&f, cudaEventDisableTiming));
+    a->ev_fork = f;
+    CUP2D_CUDA(cudaEventCreateWithFlags(&j, cudaEventDisableTiming));
+    a->ev_join = j;
+  }
+  if (!dev_dt) amr_set_dt_kernel<<<1, 1, 0, a->stream>>>(a->d_rec, dt_in);
+  CUP2D_CUDA(cudaGetLastError());
+  a->step_pending = true;
+  // the first enqueue of each form on a mesh runs directly: the lazily built tables, labs and Poisson context, the kernels'
+  // attributes and constants are set up in it (no allocation or synchronous copy may happen inside a capture)
+  const unsigned form = 1u << (2 * (a->fast ? 1 : 0) + (pressure_only ? 1 : 0));
+  bool graph = a->use_graph && (a->warmed & form);
+#ifdef CUP2D_FULL_EMU
+  graph = false;
+#endif
+  if (!graph) {
+    if ((rc = enqueue_body(a, pressure_only, dev_dt, cfl, tol_abs, tol_rel, max_restarts, max_iter, false))) return rc;
+    a->warmed |= form;
+    return CUP2D_OK;
+  }
+#ifndef CUP2D_FULL_EMU
+  auto bits = [](double v) { unsigned long long u; memcpy(&u, &v, 8); return u; };
+  const std::vector<unsigned long long> key = {(unsigned long long)a->fast, (unsigned long long)pressure_only, (unsigned long long)dev_dt,
+                                               bits(cfl), bits(tol_abs), bits(tol_rel), (unsigned long long)max_restarts,
+                                               (unsigned long long)max_iter};
+  cup2d_amr::StepGraph *hit = nullptr;
+  for (auto &g : a->graphs)
+    if (g.key == key) hit = &g;
+  if (!hit) {
+    if (a->graphs.size() >= 32) { // a caller cycling through many argument sets: drop the oldest
+      cudaGraphExecDestroy((cudaGraphExec_t)a->graphs.front().exec);
+      cudaGraphDestroy((cudaGraph_t)a->graphs.front().graph);
+      a->graphs.erase(a->graphs.begin());
+    }
+    CUP2D_CUDA(cudaStreamBeginCapture(a->stream, cudaStreamCaptureModeRelaxed));
+    rc = enqueue_body(a, pressure_only, dev_dt, cfl, tol_abs, tol_rel, max_restarts, max_iter, true);
+    cudaGraph_t g = nullptr;
+    const cudaError_t e = cudaStreamEndCapture(a->stream, &g);
+    if (rc || e != cudaSuccess) {
+      if (g) cudaGraphDestroy(g);
+      if (rc) return rc;
+      CUP2D_CUDA(e);
+    }
+    cudaGraphExec_t x = nullptr;
+    if (cudaGraphInstantiate(&x, g, 0) != cudaSuccess) {
+      cudaGraphDestroy(g);
+      set_error(std::string(who) + ": cudaGraphInstantiate failed");
+      return CUP2D_ECUDA;
+    }
+    cup2d_amr::StepGraph sg;
+    sg.key = key;
+    sg.exec = x;
+    sg.graph = g;
+    a->graphs.push_back(sg);
+    hit = &a->graphs.back();
+  }
+  CUP2D_CUDA(cudaGraphLaunch((cudaGraphExec_t)hit->exec, a->stream));
+#endif
+  return CUP2D_OK;
+}
+
+extern "C" {
+
+/* cup2d_amr_step without bodies and without host synchronisation (include/cup2d_b200.h) */
+int cup2d_amr_step_enqueue(cup2d_amr *a, double cfl, double dt_in, double tol_abs, double tol_rel, int max_restarts,
+                           int max_iter) {
+  return amr_enqueue(a, "cup2d_amr_step_enqueue", false, cfl, dt_in, tol_abs, tol_rel, max_restarts, max_iter);
+}
+
+/* the pressure section alone: poisson_rhs (u_def = tmpV, chi as they stand), solve, pressure_correct, enqueued */
+int cup2d_amr_pressure_enqueue(cup2d_amr *a, double dt, double tol_abs, double tol_rel, int max_restarts, int max_iter) {
+  return amr_enqueue(a, "cup2d_amr_pressure_enqueue", true, 0.0, dt, tol_abs, tol_rel, max_restarts, max_iter);
+}
+
+int cup2d_amr_step_result(cup2d_amr *a, double *dt_out, int *iters_out, double *err_out) {
+  CHECK_AMR(a);
+  if (!a->step_pending) {
+    set_error("cup2d_amr_step_result: no step or pressure section has been enqueued since the last result");
+    return CUP2D_ESTATE;
+  }
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  double dt = 0;
+  CUP2D_CUDA(cudaMemcpyAsync(&dt, a->d_rec + AMR_REC_DT, sizeof dt, cudaMemcpyDeviceToHost, a->stream));
+  CUP2D_CUDA(cudaStreamSynchronize(a->stream)); // (the stream waited for the solve on the Poisson context's stream)
+  a->step_pending = false;
+  const int rc = poisson_result(a->poisson, iters_out, err_out);
+  if (dt_out) *dt_out = dt;
+  return rc;
+}
+
+int cup2d_amr_set_graph(cup2d_amr *a, int on) {
+  CHECK_AMR(a);
+  if (a->dist || !a->rank_begin.empty()) {
+    set_error("cup2d_amr_set_graph: contexts on several ranks have the blocking calls only");
+    return CUP2D_ESTATE;
+  }
+  a->use_graph = on != 0;
   return CUP2D_OK;
 }
 #endif

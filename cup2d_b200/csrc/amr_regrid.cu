@@ -281,11 +281,12 @@ int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level
     set_error("cup2d_amr_regrid: transfer kernels failed");
     return fail(CUP2D_ECUDA);
   }
-  // swap: the handle takes the new mesh's internals; handle, stream, device, h0, nu and the fast flag stay
+  // swap: the handle takes the new mesh's internals; handle, stream, device, h0, nu, the fast flag and the graph switch stay
   std::swap(*a, *n);
   std::swap(a->stream, n->stream);
   a->fast = n->fast;
-  cup2d_amr_destroy(n); // the old mesh: plan, fields, tables, Poisson context, shapes
+  a->use_graph = n->use_graph;
+  cup2d_amr_destroy(n); // the old mesh: plan, fields, tables, Poisson context, shapes, the graphs of enqueued steps
   return CUP2D_OK;
 }
 

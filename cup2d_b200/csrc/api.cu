@@ -814,26 +814,15 @@ int cup2d_pressure_correct(cup2d_sim *s, double dt) {
   return launch_pressure_correct(s, dt);
 }
 
-// ---- one time step, enqueued without any host synchronisation --------------------------------------------------------
-// The body: [umax + dt rule on the device] -> RK2 -> Poisson right-hand side -> BiCGSTAB -> correction.  Every dt-dependent
-// kernel reads the device-resident StepFactors, the correction picks the best Krylov iterate through the device-side state,
-// cross-GPU epochs are device counters: nothing in the body depends on a host value that changes from step to step, so the
-// body can be captured ONCE per buffer assignment into a CUDA graph and replayed with a single cudaGraphLaunch (the
-// reference needs ~25 launches + 4 host synchronisations per Krylov iteration, cuda.cu:403-548).  A tolerance-driven solve
-// is a WHILE node whose condition the last CTA of the iteration's final kernel sets (cudaGraphSetConditional): the data-
-// dependent loop runs on the device too.
-static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, double tol_rel, int max_restarts, int max_iter,
-                     bool capturing) {
-  int rc;
-  if (dev_dt) {
-    if ((rc = launch_umax_async(s))) return rc;
-    if ((rc = launch_step_factors(s, 0.0))) return rc;
-  }
-  if ((rc = rk2(s, 0.0, s->d_fac))) return rc;
-  // keep_udef = 0: no bodies, the sum of u_def is identically zero (main.cpp:6980-6983), so the RHS
-  // kernel skips the chi*div(u_def) term instead of reading a zeroed field (tmpV keeps RK scratch).
-  // keep_udef = 1: the caller uploaded chi and the summed u_def into tmpV after the RK2 stages.
-  if ((rc = launch_pressure_rhs(s, 1.0, keep_udef != 0, s->d_fac, true))) return rc;
+} // extern "C"
+
+namespace cup2d {
+
+// The Krylov solve of an enqueued step on s->stream (b = tmp, x0 = pres; the iterate stays in the Krylov buffers, KrylovState::opt
+// names the best one).  Fixed work is queued at once; a tolerance-driven solve is, while `capturing`, a WHILE node whose
+// body is one iteration, and otherwise host-polled in batches of 8 (the only host waits, in direct launches only).
+int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current,
+                    bool capturing) {
   const bool tol = tol_abs > 0 || tol_rel > 0;
 #ifndef CUP2D_FULL_EMU
   cudaGraph_t cap_graph = nullptr;
@@ -847,7 +836,7 @@ static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, d
     s->cond_handle = (unsigned long long)handle;
   }
 #endif
-  rc = poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter, true);
+  int rc = poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter, x0_halo_current);
   if (rc) {
     s->cond_handle = 0;
     return rc;
@@ -895,6 +884,34 @@ static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, d
       }
     }
   }
+  return CUP2D_OK;
+}
+
+} // namespace cup2d
+
+extern "C" {
+
+// ---- one time step, enqueued without any host synchronisation --------------------------------------------------------
+// The body: [umax + dt rule on the device] -> RK2 -> Poisson right-hand side -> BiCGSTAB -> correction.  Every dt-dependent
+// kernel reads the device-resident StepFactors, the correction picks the best Krylov iterate through the device-side state,
+// cross-GPU epochs are device counters: nothing in the body depends on a host value that changes from step to step, so the
+// body can be captured ONCE per buffer assignment into a CUDA graph and replayed with a single cudaGraphLaunch (the
+// reference needs ~25 launches + 4 host synchronisations per Krylov iteration, cuda.cu:403-548).  A tolerance-driven solve
+// is a WHILE node whose condition the last CTA of the iteration's final kernel sets (cudaGraphSetConditional): the data-
+// dependent loop runs on the device too.
+static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, double tol_rel, int max_restarts, int max_iter,
+                     bool capturing) {
+  int rc;
+  if (dev_dt) {
+    if ((rc = launch_umax_async(s))) return rc;
+    if ((rc = launch_step_factors(s, 0.0))) return rc;
+  }
+  if ((rc = rk2(s, 0.0, s->d_fac))) return rc;
+  // keep_udef = 0: no bodies, the sum of u_def is identically zero (main.cpp:6980-6983), so the RHS
+  // kernel skips the chi*div(u_def) term instead of reading a zeroed field (tmpV keeps RK scratch).
+  // keep_udef = 1: the caller uploaded chi and the summed u_def into tmpV after the RK2 stages.
+  if ((rc = launch_pressure_rhs(s, 1.0, keep_udef != 0, s->d_fac, true))) return rc;
+  if ((rc = poisson_enqueue(s, tol_abs, tol_rel, max_restarts, max_iter, true, capturing))) return rc;
   return launch_pressure_correct(s, 1.0, s->d_fac, true);
 }
 

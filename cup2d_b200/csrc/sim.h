@@ -200,6 +200,9 @@ int poisson_solve(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts
 int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current);
 int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream);
 int poisson_result(cup2d_sim *s, int *iters, double *err);
+// begin + iterations of an enqueued solve (csrc/api.cu): a WHILE node while capturing a tolerance-driven solve, else launches
+int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current,
+                    bool capturing);
 int halo_exchange_ptr(cup2d_sim *s, double *base, int dim, int peer_index, bool done_barrier = true);
 int halo_exchange_xopt(cup2d_sim *s); // halo of the x buffer KrylovState::opt names (chosen on the device)
 int comm_check(cup2d_sim *s);         // CUP2D_ECOMM if a cross-GPU wait of this rank was given up

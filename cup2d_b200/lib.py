@@ -33,6 +33,7 @@ SYMBOLS = [
     "cup2d_amr_adapt_mesh", "cup2d_amr_regrid", "cup2d_amr_ongrid", "cup2d_amr_shape_get",
     "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times", "cup2d_amr_shape_set_dist", "cup2d_amr_collide",
     "cup2d_amr_surface", "cup2d_amr_surface_get", "cup2d_amr_forces", "cup2d_amr_udef_blend",
+    "cup2d_amr_step_enqueue", "cup2d_amr_pressure_enqueue", "cup2d_amr_step_result", "cup2d_amr_set_graph",
 ]
 
 
@@ -155,6 +156,10 @@ def load_library():
     lib.cup2d_amr_poisson_solve.argtypes = [P, D, D, I, I, C.POINTER(I), C.POINTER(D)]
     lib.cup2d_amr_pressure_correct.argtypes = [P, D]
     lib.cup2d_amr_step.argtypes = [P, D, D, D, D, I, I, C.POINTER(D), C.POINTER(I), C.POINTER(D)]
+    lib.cup2d_amr_step_enqueue.argtypes = [P, D, D, D, D, I, I]
+    lib.cup2d_amr_pressure_enqueue.argtypes = [P, D, D, D, I, I]
+    lib.cup2d_amr_step_result.argtypes = [P, C.POINTER(D), C.POINTER(I), C.POINTER(D)]
+    lib.cup2d_amr_set_graph.argtypes = [P, I]
     lib.cup2d_amr_shape_set.argtypes = [P, I, I, P, P, P]
     lib.cup2d_amr_shape_integrals.argtypes = [P, I, D, D, D, D, C.POINTER(D)]
     lib.cup2d_amr_penalize.argtypes = [P, I, D, D, D, D, D, D, D]

@@ -310,6 +310,24 @@ int cup2d_amr_poisson_solve(cup2d_amr *a, double tol_abs, double tol_rel, int ma
 int cup2d_amr_pressure_correct(cup2d_amr *a, double dt);
 int cup2d_amr_step(cup2d_amr *a, double cfl, double dt_in, double tol_abs, double tol_rel, int max_restarts, int max_iter,
                    double *dt_out, int *iters, double *err);
+/* Enqueued forms, without host synchronisation (one GPU, single-rank contexts only: contexts of cup2d_amr_set_ranks or
+ * cup2d_amr_create_ranks return CUP2D_ESTATE).  dt, the two pressure means and the Krylov stopping rule stay on the device;
+ * from the second enqueue of a form on a mesh, each enqueue is one CUDA graph launch (one graph per argument set, rebuilt
+ * after cup2d_amr_regrid).  Several enqueues may come before one result.  Bad arguments return CUP2D_EINVAL with the
+ * context untouched.  dt equals cup2d_amr_compute_dt's bit for bit; the means are summed in a fixed order on the device
+ * (DESIGN.md 7.1), so fields agree with the blocking calls to rounding.
+ * cup2d_amr_step_enqueue: cup2d_amr_step (no bodies); dt_in <= 0 runs the dt rule of cup2d_amr_compute_dt with cfl on the
+ * device. */
+int cup2d_amr_step_enqueue(cup2d_amr *a, double cfl, double dt_in, double tol_abs, double tol_rel, int max_restarts, int max_iter);
+/* the pressure section alone, for loops with bodies (call after cup2d_amr_udef_assemble): cup2d_amr_poisson_rhs with
+ * u_def = tmpV and chi as they stand, the solve, cup2d_amr_pressure_correct; dt > 0 */
+int cup2d_amr_pressure_enqueue(cup2d_amr *a, double dt, double tol_abs, double tol_rel, int max_restarts, int max_iter);
+/* waits for the last enqueued step / pressure section: dt used, Krylov iterations, residual (any pointer may be NULL);
+ * CUP2D_ESTATE if nothing was enqueued since the last result */
+int cup2d_amr_step_result(cup2d_amr *a, double *dt_out, int *iters_out, double *err_out);
+/* on = 0: every enqueue launches its kernels directly (profiling; a tolerance-driven solve is then host-polled every 8
+ * iterations); default 1 */
+int cup2d_amr_set_graph(cup2d_amr *a, int on);
 
 /* Several GPUs (first form): every rank creates the context over the WHOLE mesh and computes the stencil operators
  * redundantly — bitwise the same on every rank — while the Poisson solve is distributed over the ranks by the block ranges
