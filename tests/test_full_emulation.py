@@ -389,6 +389,60 @@ assert worst < 1e-11
     assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
 
 
+def test_distributed_generated_mesh_in_random_order_emulated(emulated_library):
+    """the distributed form (cup2d_amr_create_ranks) on a generated 1x3 mesh (tests/amr_meshes.py) listed in random order, on 2
+    and on 3 ranks: contiguous rank ranges of a shuffled list put coarse-fine faces, wall ghosts and Poisson couplings across
+    rank boundaries all over the mesh.  Two full steps against the one-rank context, with the bound of the three-rank test
+    above."""
+    code = r'''
+import sys, threading, numpy as np
+sys.path.insert(0, %r); sys.path.insert(0, %r); sys.path.insert(0, %r)
+import amr_meshes
+from cup2d_b200.amr import AmrSimulation
+bx, by, blocks, _ = amr_meshes.GENERATED["1x3_mixed"]
+mb = amr_meshes.order(blocks, bx, by, "random"); mn = len(mb); h0 = 1 / 8
+rng = np.random.default_rng(7)
+vel, pres = rng.uniform(-1, 1, (mn, 8, 8, 2)), rng.uniform(-1, 1, (mn, 8, 8, 1))
+def steps(sim, sl):
+    out = []
+    sim.upload("vel", vel[sl]); sim.upload("pres", pres[sl])
+    for s in range(2):
+        info = sim.step(cfl=0.5, max_iter=5)
+        out.append((info, sim.download("vel"), sim.download("pres")))
+    return out
+one = AmrSimulation(mb, bx, by, h0, 1e-3); one.set_fast(True); ref = steps(one, slice(0, mn)); one.close()
+worst = 0.0
+for W in (2, 3):
+    bar, slots, errs = threading.Barrier(W), [None] * W, []
+    class Dist:
+        def __init__(self, rank): self.rank = rank
+        def all_gather_object(self, out, obj):
+            slots[self.rank] = obj; bar.wait(); out[:] = slots; bar.wait()
+        def barrier(self): bar.wait()
+    rb = [mn * r // W + (5 if 0 < r < W else 0) for r in range(W + 1)]
+    res = [None] * W
+    def run(rank):
+        try:
+            sim = AmrSimulation.distributed(mb, bx, by, h0, 1e-3, rank, rb, Dist(rank))
+            res[rank] = steps(sim, slice(rb[rank], rb[rank + 1])); bar.wait(); sim.close()
+        except Exception as e:
+            errs.append(repr(e)); bar.abort()
+    ths = [threading.Thread(target=run, args=(r,)) for r in range(W)]
+    [t.start() for t in ths]; [t.join() for t in ths]
+    assert not errs, errs
+    for s in range(2):
+        v = np.concatenate([res[r][s][1] for r in range(W)]); p = np.concatenate([res[r][s][2] for r in range(W)])
+        worst = max(worst, np.abs(v - ref[s][1]).max() / np.abs(ref[s][1]).max(), np.abs(p - ref[s][2]).max() / np.abs(ref[s][2]).max(),
+                    abs(res[0][s][0][0] - ref[s][0][0]) / ref[s][0][0])
+        assert all(res[r][s][0] == res[0][s][0] for r in range(W)) and res[0][s][0][1] == ref[s][0][1] == 5
+print("WORST", worst)
+assert worst < 1e-11
+''' % (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests"))
+    r = subprocess.run([sys.executable, "-c", code], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600,
+                       env=dict(os.environ, CUP2D_B200_LIB=emulated_library))
+    assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
+
+
 # The two sanitizer builds recompile every product source with -fsanitize and take 4-6 minutes on 8 cores: they run when asked
 # for (CUP2D_TEST_SANITIZERS=1, as tools/run_emulated_gpu_tests.sh does); the hardware counterpart is compute-sanitizer
 # memcheck/racecheck on a GPU.
