@@ -264,14 +264,28 @@ class AmrSimulation:
         _l.check(self.lib.cup2d_amr_regrid(self._h, len(b), b.ctypes.data_as(C.POINTER(C.c_int32))))
         self.blocks = b.copy()
 
-    def adapt(self, rtol, ctol, level_max):
-        """adapt() on the device-resident fields: tags -> decision -> regrid; returns whether the mesh changed"""
-        linf = self.adapt_tags(rtol, level_max)
-        new = adapt_mesh(self.blocks, self.bpdx, self.bpdy, level_max, linf, rtol, ctol)
-        if np.array_equal(new, self.blocks):
-            return False
-        self.regrid(new)
-        return True
+    def adapt(self, rtol, ctol, level_max, block_linf=None):
+        """adapt() on the device-resident fields in one call (cup2d_amr_adapt): tags (or the caller's per-block `block_linf`),
+        decision, order and transfer on the device, the same mesh and fields as adapt_tags -> adapt_mesh -> regrid; returns
+        whether the mesh changed"""
+        linf = None
+        if block_linf is not None:
+            linf = np.ascontiguousarray(block_linf, dtype=np.float64)
+            assert linf.shape == (len(self.blocks),)
+        changed = C.c_int32()
+        _l.check(self.lib.cup2d_amr_adapt(self._h, None if linf is None else linf.ctypes.data_as(C.POINTER(C.c_double)),
+                                          float(rtol), float(ctol), int(level_max), None, C.byref(changed)))
+        self.blocks = self.block_list()
+        return bool(changed.value)
+
+    def block_list(self):
+        """the context's current block list, [n][3] (level, i, j) (cup2d_amr_blocks)"""
+        n = self.lib.cup2d_amr_blocks(self._h, None)
+        if n < 0:
+            _l.check(int(n))
+        out = np.empty((n, 3), dtype=np.int32)
+        self.lib.cup2d_amr_blocks(self._h, out.ctypes.data_as(C.POINTER(C.c_int32)))
+        return out
 
     # ---- bodies (cup2d_amr_shape_*): the calls of Simulation.shape_* on the multi-level context ----
     def shape_set(self, shape, ids, X, udef):

@@ -81,6 +81,9 @@ int amr_plan_subset_rows(cup2d_amr_plan *p, int which, int64_t nsub, const int32
                          std::vector<int32_t> &src_block, std::vector<int32_t> &src_cellcomp, std::vector<double> &weight);
 
 struct cup2d_amr;
+// adapt()'s tagging (cup2d_amr_adapt_tags) enqueued on the context's stream: the tagging field in tmp, the per-block L-inf in
+// d_part[0..nb) (csrc/amr_ops.cu)
+extern "C" int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max);
 // single-rank contexts: the fast path's neighbour / irregular-block / compact ghost tables (csrc/amr_fast.cu), built on first use
 int amr_fast_tables(cup2d_amr *a);
 // the per-block (i, j) table on the device, built on first use (csrc/amr_penalize.cu)

@@ -555,12 +555,7 @@ static int block_partials(cup2d_amr *a, int n_per_block) {
 /* adapt()'s per-block L-inf (main.cpp:4676-4697) on a multi-level mesh: vorticity of vel through the +-1 lab, the chi rule
  * of GradChiOnTmp through the {-4,-4,5,5,tensorial} chi lab (ghost tables built on first use); leaves the tagging field in
  * tmp like the reference does.  level_max = sim.levelMax (the finest level is level_max - 1). */
-int cup2d_amr_adapt_tags(cup2d_amr *a, double rtol, int level_max, double *block_linf_out) {
-  CHECK_AMR(a);
-  if (!block_linf_out || level_max < 1 || level_max > 30) {
-    set_error("cup2d_amr_adapt_tags: bad arguments");
-    return CUP2D_EINVAL;
-  }
+int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max) {
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc;
   if ((rc = amr_dist_refresh(a, CUP2D_VEL)) || (rc = amr_dist_refresh(a, CUP2D_CHI))) return rc;
@@ -569,7 +564,17 @@ int cup2d_amr_adapt_tags(cup2d_amr *a, double rtol, int level_max, double *block
   amr_tag_block_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->lab[3], a->f[CUP2D_TMP], a->d_h,
                                                                a->h0 / (double)(1 << (level_max - 1)), rtol, a->d_part, a->nb);
   CUP2D_CUDA(cudaGetLastError());
-  if ((rc = block_partials(a, 1))) return rc;
+  return CUP2D_OK;
+}
+
+int cup2d_amr_adapt_tags(cup2d_amr *a, double rtol, int level_max, double *block_linf_out) {
+  CHECK_AMR(a);
+  if (!block_linf_out || level_max < 1 || level_max > 30) {
+    set_error("cup2d_amr_adapt_tags: bad arguments");
+    return CUP2D_EINVAL;
+  }
+  int rc;
+  if ((rc = amr_adapt_tags_enqueue(a, rtol, level_max)) || (rc = block_partials(a, 1))) return rc;
   memcpy(block_linf_out, a->h_part.data(), (size_t)a->nb * sizeof(double));
   return CUP2D_OK;
 }

@@ -14,6 +14,7 @@
 // the row mix-up in the fine->coarse average across x faces (main.cpp:2529-2530) and the Taylor ghosts of a vector lab
 // taking component 0 for every component (main.cpp:2751-2765); see DESIGN.md 7.1.
 #include "../../include/cup2d_b200.h"
+#include "curve.h"
 #include <algorithm>
 #include <array>
 #include <cstdlib>
@@ -881,86 +882,13 @@ int cup2d_amr_plan_neighbours(cup2d_amr_plan *p, int32_t *out) {
 }
 
 /* ---- adapt()'s refine / compress decision (main.cpp:4676-4860) and the order of the new block list (fill_pos, Encode:
- * main.cpp:1550-1553, 422-445, SpaceCurve 342-421 and 6342-6376).  Host only: a pure function of the block list and the
- * per-block L-inf of the tagging field (cup2d_amr_adapt_tags).  The states are updated in place in the reference's loop
+ * main.cpp:1550-1553, 422-445, SpaceCurve 342-421 and 6342-6376; csrc/curve.h).  A pure function of the block list and
+ * the per-block L-inf of the tagging field (cup2d_amr_adapt_tags).  The states are updated in place in the reference's loop
  * order (blocks in list order, levels from levelMax-1 down), so the result is the reference's, order effects included.
+ * cup2d_amr_adapt (csrc/amr_regrid.cu) makes the same decision on the device and must return the same list.
  * Neighbour positions outside the domain are skipped; the reference wraps their index, which differs only on a level with a
  * single block row or column. */
 namespace {
-struct Curve { // SpaceCurve::forward / inverse / Encode
-  int bpdx, bpdy, lmax, base = 0;
-  bool regular = true;
-  std::vector<int64_t> zsave;            // [j * bpdx + i]
-  std::vector<std::array<int, 2>> inv;   // zsave value -> (i, j)
-  static int64_t xy2d(int b, int x, int y) {
-    const int n = 1 << b;
-    int64_t d = 0;
-    for (int s = n / 2; s > 0; s /= 2) {
-      const int rx = (x & s) > 0, ry = (y & s) > 0;
-      d += (int64_t)s * s * ((3 * rx) ^ ry);
-      if (ry == 0) {
-        if (rx == 1) x = n - 1 - x, y = n - 1 - y;
-        std::swap(x, y);
-      }
-    }
-    return d;
-  }
-  static void d2xy(int b, int64_t t, int &x, int &y) {
-    const int n = 1 << b;
-    x = y = 0;
-    for (int64_t s = 1; s < n; s *= 2) {
-      const int64_t rx = 1 & (t / 2), ry = 1 & (t ^ rx);
-      if (ry == 0) {
-        if (rx == 1) x = (int)s - 1 - x, y = (int)s - 1 - y;
-        std::swap(x, y);
-      }
-      x += (int)(s * rx), y += (int)(s * ry);
-      t /= 4;
-    }
-  }
-  Curve(int bx, int by, int lm) : bpdx(bx), bpdy(by), lmax(lm), zsave((size_t)bx * by), inv((size_t)bx * by) {
-    while ((1 << base) < std::max(bx, by)) base++;
-    for (int j = 0; j < by; j++)
-      for (int i = 0; i < bx; i++) {
-        int64_t index = xy2d(base, i, j), sub = 0;
-        for (int64_t h = 0; h < index; h++) {
-          int x, y;
-          d2xy(base, h, x, y);
-          sub += x >= bx || y >= by;
-        }
-        if (sub) regular = false;
-        zsave[(size_t)j * bx + i] = index - sub;
-        inv[index - sub] = {i, j};
-      }
-  }
-  int64_t forward(int l, int i, int j) const {
-    if (l >= lmax) return 0;
-    if (regular) return xy2d(l + base, i, j);
-    const int aux = 1 << l, I = i / aux, J = j / aux;
-    return xy2d(l, i - I * aux, j - J * aux) + zsave[(size_t)J * bpdx + I] * aux * aux;
-  }
-  void inverse(int64_t Z, int l, int &i, int &j) const {
-    if (regular) return d2xy(l + base, Z, i, j);
-    const int64_t aux = 1LL << l;
-    d2xy(l, Z % (aux * aux), i, j);
-    const auto &IJ = inv[(size_t)(Z / (aux * aux))];
-    i += IJ[0] * (int)aux, j += IJ[1] * (int)aux;
-  }
-  int64_t encode(int level, int i, int j) const {
-    int64_t r = 0;
-    for (int l = level, ix = i, iy = j; l >= 0; l--, ix /= 2, iy /= 2) r += forward(l, ix, iy);
-    int ix = 2 * i, iy = 2 * j;
-    for (int l = level + 1; l < lmax; l++) {
-      int64_t Zc = forward(l, ix, iy);
-      Zc -= Zc % 4;
-      r += Zc;
-      int ix1, iy1;
-      inverse(Zc, l, ix1, iy1);
-      ix = 2 * ix1, iy = 2 * iy1;
-    }
-    return r + level;
-  }
-};
 enum { LEAVE = 0, REFINE = 1, COMPRESS = 2 };
 } // namespace
 
@@ -1062,7 +990,8 @@ int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t b
       out.push_back({l, i, j});
   }
   if (new_level_ij) {
-    const Curve curve(bpdx, bpdy, level_max);
+    const cup2d::CurveTables tables(bpdx, bpdy);
+    const cup2d::Curve curve = tables.curve(level_max);
     std::vector<std::pair<int64_t, size_t>> key(out.size());
     for (size_t q = 0; q < out.size(); q++) key[q] = {curve.encode(out[q][0], out[q][1], out[q][2]), q};
     std::sort(key.begin(), key.end());

@@ -13,6 +13,8 @@
 // Then the context swaps its internals for those of the new mesh: plan, cell sizes, coarse faces, block index tables, lab
 // buffers and Poisson context (rebuilt lazily on first use, as after cup2d_amr_create); shapes are cleared, their block ids
 // naming old blocks.  Handle, stream, device, h0, nu and the fast flag are kept.  Peak memory: old plus new fields.
+// cup2d_amr_adapt adds adapt()'s refine / compress decision and the order of the new list on the device (the kernels below
+// the transfer's), and feeds the same transfer (regrid_apply) from the device without cup2d_amr_regrid's host classification.
 #include "sim.h"
 #include <algorithm>
 #include <array>
@@ -21,6 +23,7 @@
 #include <vector>
 
 #include "amr.h"
+#include "curve.h"
 
 namespace cup2d {
 
@@ -137,7 +140,339 @@ __global__ void amr_regrid_refine_kernel(RgFields F, RgLab L, const int *__restr
   }
 }
 
+// ---- adapt()'s decision on the device (cup2d_amr_adapt): cup2d_amr_adapt_mesh (csrc/amr_plan.cpp) kernel by kernel ------
+// The old mesh is looked up through its (level, i, j) keys sorted with the block ids (AdIndex: binary search; state() walks
+// up the ancestors as Mesh::state does).  The host updates the states in place in the reference's loop order; the kernels
+// below run every block of a pass at once and still give the host's answer, because no pass reads what it writes:
+//   - the finer-neighbour pass at level lv (amr_plan.cpp: main.cpp:4735-4785) reads the states of level lv+1 only, final
+//     after that level's passes, and writes the states of level lv only;
+//   - the same-level pass (main.cpp:4791-4823) reads `== REFINE` of level lv and turns COMPRESS into LEAVE only, so no write
+//     changes what another block reads; it reads one state array and writes another all the same;
+//   - the sibling pass (main.cpp:4825-4860) is idempotent within each group of four: a group whose four states are COMPRESS
+//     is left alone, every other group loses all its COMPRESS states whichever member is visited first.  Each block writes
+//     its own state into a second array from the group as it was.
+// Levels are processed from level_max-1 down to 0, one launch per pass and level, as the host's outer loop.  Neighbour
+// enumeration uses the host's order and skip rules (skin skips; positions outside the domain skipped, not wrapped).
+enum { AD_LEAVE = 0, AD_REFINE = 1, AD_COMPRESS = 2 };
+typedef unsigned long long u64;
+
+// (l, i, j) -> sortable key; l <= 20 and i, j < 2^29 (checked before the decision)
+__device__ __forceinline__ u64 ad_key(int l, int i, int j) { return ((u64)l << 58) | ((u64)i << 29) | (u64)j; }
+
+struct AdIndex {           // the old mesh: keys sorted ascending with their block ids
+  const u64 *key;
+  const int *id;
+  int64_t n;
+  __device__ int find(int l, int i, int j) const {
+    const u64 k = ad_key(l, i, j);
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (key[mid] < k) lo = mid + 1;
+      else hi = mid;
+    }
+    return lo < n && key[lo] == k ? id[lo] : -1;
+  }
+  __device__ int state(int l, int i, int j) const { // Mesh::state: >= 0 block id, -1 refined further, -2 covered by a coarser block
+    const int k = find(l, i, j);
+    if (k >= 0) return k;
+    while (l > 0) {
+      l--, i >>= 1, j >>= 1;
+      if (find(l, i, j) >= 0) return -2;
+    }
+    return -1;
+  }
+};
+
+struct AdMesh {
+  const int *lij;          // [n][3] old blocks
+  AdIndex idx;
+  int bpdx, bpdy, level_max;
+  int64_t n;
+};
+
+// the host's `neighbours` skip rules: (x, y) is not visited from block (I, J) of an NX x NY level
+__device__ __forceinline__ bool ad_skip(int x, int y, int I, int J, int NX, int NY) {
+  const bool xskin = I == 0 || I == NX - 1, yskin = J == 0 || J == NY - 1;
+  const int xskip = I == 0 ? -1 : 1, yskip = J == 0 ? -1 : 1;
+  return (x == 0 && y == 0) || (x == xskip && xskin) || (y == yskip && yskin) || I + x < 0 || I + x >= NX || J + y < 0 ||
+         J + y >= NY;
+}
+
+// (key, id) of every old block; the tail up to the power of two `npad` sorts last
+__global__ void amr_adapt_index_kernel(const int *__restrict__ lij, u64 *key, int *id, int64_t n, int64_t npad) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < npad; k += (int64_t)gridDim.x * blockDim.x) {
+    key[k] = k < n ? ad_key(lij[3 * k], lij[3 * k + 1], lij[3 * k + 2]) : ~0ull;
+    id[k] = k < n ? (int)k : 0x7fffffff;
+  }
+}
+
+// one compare-exchange pass (k, j) of a bitonic sort of (key, val) pairs into ascending (key, val) order; n a power of two.
+// Launched log2(n) (log2(n) + 1) / 2 times; thread i owns the pair (i, i ^ j) with i < i ^ j, so a pass has no conflicts.
+__global__ void amr_adapt_bitonic_kernel(u64 *key, int *val, int64_t n, int64_t k, int64_t j) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i ^ j;
+    if (p <= i) continue;
+    const u64 ki = key[i], kp = key[p];
+    const int vi = val[i], vp = val[p];
+    const bool greater = ki > kp || (ki == kp && vi > vp);
+    if (greater == ((i & k) == 0)) {
+      key[i] = kp, key[p] = ki;
+      val[i] = vp, val[p] = vi;
+    }
+  }
+}
+
+// thresholds (main.cpp:4682-4688): no Refine at level_max-1, no Compress at level 0
+__global__ void amr_adapt_state_kernel(AdMesh M, const double *__restrict__ linf, double rtol, double ctol, int *st) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int l = M.lij[3 * k];
+    int s = linf[k] > rtol ? AD_REFINE : linf[k] < ctol ? AD_COMPRESS : AD_LEAVE;
+    if ((s == AD_REFINE && l == M.level_max - 1) || (s == AD_COMPRESS && l == 0)) s = AD_LEAVE;
+    st[k] = s;
+  }
+}
+
+// finer neighbours (main.cpp:4735-4785) of the blocks of level lv: in place, reads level lv+1, writes level lv
+__global__ void amr_adapt_finer_kernel(AdMesh M, int *st, int lv) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int l = M.lij[3 * k], I = M.lij[3 * k + 1], J = M.lij[3 * k + 2];
+    if (l != lv || st[k] == AD_REFINE || l == M.level_max - 1) continue;
+    const int NX = M.bpdx << l, NY = M.bpdy << l;
+    int s = st[k];
+    bool done = false;
+    for (int x = -1; x < 2 && !done; x++)
+      for (int y = -1; y < 2 && !done; y++) {
+        if (ad_skip(x, y, I, J, NX, NY) || M.idx.state(l, I + x, J + y) != -1) continue;
+        if (s == AD_COMPRESS) s = AD_LEAVE;
+        const int Bstep = abs(x) + abs(y) == 2 ? 3 : 1;
+        for (int B = 0; B <= 1; B += Bstep) {
+          const int aux = abs(x) == 1 ? B % 2 : B / 2;
+          const int iN = 2 * I + (x > 0 ? x : 0) + x + (B % 2) * (1 - abs(x)); // |x|, |y| <= 1: max(0, 1-|x|) = 1-|x|
+          const int jN = 2 * J + (y > 0 ? y : 0) + y + aux * (1 - abs(y));
+          const int q = M.idx.find(lv + 1, iN, jN);
+          if (q >= 0 && st[q] == AD_REFINE) {
+            s = AD_REFINE;
+            done = true;
+            break;
+          }
+        }
+      }
+    st[k] = s;
+  }
+}
+
+// a same-level neighbour refines (main.cpp:4791-4823): level lv from `in` into `out`, every other state copied
+__global__ void amr_adapt_same_kernel(AdMesh M, const int *__restrict__ in, int *__restrict__ out, int lv) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int l = M.lij[3 * k], I = M.lij[3 * k + 1], J = M.lij[3 * k + 2];
+    int s = in[k];
+    if (l == lv && s == AD_COMPRESS) {
+      const int NX = M.bpdx << l, NY = M.bpdy << l;
+      for (int x = -1; x < 2 && s == AD_COMPRESS; x++)
+        for (int y = -1; y < 2; y++) {
+          if (ad_skip(x, y, I, J, NX, NY)) continue;
+          const int q = M.idx.find(l, I + x, J + y);
+          if (q >= 0 && in[q] == AD_REFINE) {
+            s = AD_LEAVE;
+            break;
+          }
+        }
+    }
+    out[k] = s;
+  }
+}
+
+// all four siblings compress, or none does (main.cpp:4825-4860): from `in` into `out`
+__global__ void amr_adapt_siblings_kernel(AdMesh M, const int *__restrict__ in, int *__restrict__ out) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    int s = in[k];
+    if (s == AD_COMPRESS) {
+      const int l = M.lij[3 * k], i0 = 2 * (M.lij[3 * k + 1] / 2), j0 = 2 * (M.lij[3 * k + 2] / 2);
+      for (int a = 0; a < 2; a++)
+        for (int b = 0; b < 2; b++) {
+          const int q = M.idx.find(l, i0 + a, j0 + b);
+          if (q < 0 || in[q] != AD_COMPRESS) s = AD_LEAVE;
+        }
+    }
+    out[k] = s;
+  }
+}
+
+// what old block k contributes: (new blocks, copy pairs, refined parents, compressed groups)
+__device__ __forceinline__ int4 ad_count(int s, int i, int j) {
+  if (s == AD_REFINE) return make_int4(4, 0, 1, 0);
+  if (s == AD_COMPRESS) return i % 2 == 0 && j % 2 == 0 ? make_int4(1, 0, 0, 1) : make_int4(0, 0, 0, 0);
+  return make_int4(1, 1, 0, 0);
+}
+__global__ void amr_adapt_count_kernel(AdMesh M, const int *__restrict__ st, int4 *cnt) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x)
+    cnt[k] = ad_count(st[k], M.lij[3 * k + 1], M.lij[3 * k + 2]);
+}
+
+// one step (distance d) of an inclusive Hillis-Steele scan of the four counts; launched log2(n) times, ping-pong
+__global__ void amr_adapt_scan_kernel(const int4 *__restrict__ in, int4 *__restrict__ out, int64_t n, int64_t d) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
+    int4 v = in[k];
+    if (k >= d) {
+      const int4 u = in[k - d];
+      v.x += u.x, v.y += u.y, v.z += u.z, v.w += u.w;
+    }
+    out[k] = v;
+  }
+}
+
+// the new blocks in the host's emission order (main.cpp:4926-5195) at the exclusive offsets, with their Encode keys and
+// emission indices for the sort (keys padded to the power of two `npad`); the refined parents in old-block order
+__global__ void amr_adapt_emit_kernel(AdMesh M, const int *__restrict__ st, const int4 *__restrict__ incl, Curve curve,
+                                      int *out_lij, u64 *key, int *val, int64_t nnew, int64_t npad, int *parents) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int l = M.lij[3 * k], i = M.lij[3 * k + 1], j = M.lij[3 * k + 2], s = st[k];
+    const int4 c = ad_count(s, i, j), e = incl[k];
+    int q = e.x - c.x;
+    auto put = [&](int nl, int ni, int nj) {
+      out_lij[3 * q] = nl, out_lij[3 * q + 1] = ni, out_lij[3 * q + 2] = nj;
+      key[q] = (u64)curve.encode(nl, ni, nj);
+      val[q] = q;
+      q++;
+    };
+    if (s == AD_REFINE) {
+      for (int b = 0; b < 2; b++)
+        for (int a = 0; a < 2; a++) put(l + 1, 2 * i + a, 2 * j + b);
+      parents[e.z - 1] = (int)k;
+    } else if (c.x) {
+      if (s == AD_COMPRESS) put(l - 1, i / 2, j / 2);
+      else put(l, i, j);
+    }
+  }
+  for (int64_t q = nnew + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < npad; q += (int64_t)gridDim.x * blockDim.x)
+    key[q] = ~0ull, val[q] = 0x7fffffff;
+}
+
+// sorted position p -> new block list, and emission index -> p
+__global__ void amr_adapt_rank_kernel(const int *__restrict__ val, const int *__restrict__ out_lij, int *new_lij, int *rank,
+                                      int64_t nnew) {
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < nnew; p += (int64_t)gridDim.x * blockDim.x) {
+    const int q = val[p];
+    rank[q] = (int)p;
+    for (int c = 0; c < 3; c++) new_lij[3 * p + c] = out_lij[3 * q + c];
+  }
+}
+
+// the transfer's inputs, as cup2d_amr_regrid classifies them: copy pairs, the new positions of the children of every
+// refined parent, the compressed groups (their sibling ids from the index, J*2 + I order)
+__global__ void amr_adapt_transfer_kernel(AdMesh M, const int *__restrict__ st, const int4 *__restrict__ incl,
+                                          const int *__restrict__ rank, int2 *pairs, int *child_dst, int4 *kids, int *cdst) {
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < M.n; k += (int64_t)gridDim.x * blockDim.x) {
+    const int l = M.lij[3 * k], i = M.lij[3 * k + 1], j = M.lij[3 * k + 2], s = st[k];
+    const int4 c = ad_count(s, i, j), e = incl[k];
+    const int q = e.x - c.x;
+    if (c.y) pairs[e.y - 1] = make_int2(rank[q], (int)k);
+    if (c.z)
+      for (int t = 0; t < 4; t++) child_dst[4 * (e.z - 1) + t] = rank[q + t];
+    if (c.w) {
+      cdst[e.w - 1] = rank[q];
+      kids[e.w - 1] = make_int4((int)k, M.idx.find(l, i + 1, j), M.idx.find(l, i, j + 1), M.idx.find(l, i + 1, j + 1));
+    }
+  }
+}
+
 static int rg_grid(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, AMR_GRID_SMS * 16)); }
+
+// device buffers of one call, freed with it
+struct RgScratch {
+  std::vector<void *> p;
+  bool ok = true;
+  template <class T> T *get(size_t n) {
+    T *d = nullptr;
+    if (cudaMalloc(&d, std::max<size_t>(n, 1) * sizeof(T)) != cudaSuccess) {
+      ok = false;
+      return nullptr;
+    }
+    p.push_back((void *)d);
+    return d;
+  }
+  template <class T> T *up(const std::vector<T> &h) {
+    T *d = get<T>(h.size());
+    if (d && !h.empty() && cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) ok = false;
+    return d;
+  }
+  ~RgScratch() {
+    for (void *q : p) cudaFree(q);
+  }
+};
+
+static int64_t pow2_at_least(int64_t n) {
+  int64_t m = 1;
+  while (m < n) m <<= 1;
+  return m;
+}
+
+static void bitonic_sort(cudaStream_t stream, u64 *key, int *val, int64_t n) {
+  for (int64_t k = 2; k <= n; k <<= 1)
+    for (int64_t j = k >> 1; j > 0; j >>= 1) amr_adapt_bitonic_kernel<<<rg_grid(n), 256, 0, stream>>>(key, val, n, k, j);
+}
+
+// The transfer and the swap of a regrid whose classification is on the device (see the head of this file): copy pairs
+// (new block, old block), compressed groups (kids[g] -> cdst[g]) and refined parents (children child_dst[4 q + J*2 + I]);
+// `parents` (host, any order, matching child_dst) selects the lab rows, new_level_ij[nnew][3] the new context's mesh.
+static int regrid_apply(cup2d_amr *a, const char *who, int64_t nnew, const int32_t *new_level_ij, int bpdx, int bpdy,
+                        const std::vector<int32_t> &parents, const int2 *d_pairs, int64_t np, const int4 *d_kids,
+                        const int *d_cdst, int64_t ng, const int *d_child) {
+  // the new context (plan = 2:1 check, zeroed fields, cell sizes, coarse faces); the old one stays valid until the swap
+  cup2d_amr *n = nullptr;
+  int rc = cup2d_amr_create(nnew, new_level_ij, bpdx, bpdy, a->h0, a->nu, a->device, &n);
+  if (rc) return rc;
+  auto fail = [&](int code) {
+    cup2d_amr_destroy(n);
+    return code;
+  };
+  // lab rows of the refined parents on the old mesh (kind 4: vector, 5: scalar)
+  std::vector<int64_t> rp[2];
+  std::vector<int32_t> sb[2], sc[2];
+  std::vector<double> w[2];
+  for (int k = 0; k < 2; k++)
+    if ((rc = amr_plan_subset_rows(a->plan, 4 + k, (int64_t)parents.size(), parents.data(), rp[k], sb[k], sc[k], w[k]))) return fail(rc);
+  const int fields[RG_NF] = {CUP2D_TMP, CUP2D_CHI, CUP2D_VEL, CUP2D_VOLD, CUP2D_PRES, CUP2D_POLD};
+  RgFields F;
+  F.off2[0] = 0;
+  for (int f = 0; f < RG_NF; f++) {
+    F.src[f] = a->f[fields[f]], F.dst[f] = n->f[fields[f]], F.dim[f] = dim_of(fields[f]);
+    F.off2[f + 1] = F.off2[f] + 32 * F.dim[f];
+  }
+  const int64_t nq = (int64_t)parents.size();
+  bool launched;
+  {
+    RgScratch S;
+    RgLab L = {};
+    for (int k = 0; k < 2; k++) L.rowptr[k] = S.up(rp[k]), L.sb[k] = S.up(sb[k]), L.sc[k] = S.up(sc[k]), L.w[k] = S.up(w[k]);
+    L.rbeg[0] = 0;
+    for (int f = 0; f < RG_NF; f++) L.rbeg[f + 1] = L.rbeg[f] + (int64_t)rp[F.dim[f] == 2 ? 0 : 1].size() - 1;
+    for (int f = 0; f < RG_NF; f++) L.lab[f] = S.get<double>((size_t)nq * 100 * F.dim[f]);
+    if (!S.ok) {
+      set_error(std::string(who) + ": out of device memory");
+      return fail(CUP2D_ECUDA);
+    }
+    if (np) amr_regrid_copy_kernel<<<rg_grid(np * F.off2[RG_NF]), 256, 0, a->stream>>>(F, d_pairs, np);
+    if (ng) amr_regrid_compress_kernel<<<rg_grid(ng * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, d_cdst, d_kids, ng);
+    if (nq) {
+      amr_regrid_lab_kernel<<<rg_grid(L.rbeg[RG_NF]), 256, 0, a->stream>>>(F, L);
+      amr_regrid_refine_kernel<<<rg_grid(nq * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, L, d_child, nq);
+    }
+    launched = cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(a->stream) == cudaSuccess;
+  }
+  if (!launched) {
+    set_error(std::string(who) + ": transfer kernels failed");
+    return fail(CUP2D_ECUDA);
+  }
+  // swap: the handle takes the new mesh's internals; handle, stream, device, h0, nu, the fast flag and the graph switch stay
+  std::swap(*a, *n);
+  std::swap(a->stream, n->stream);
+  a->fast = n->fast;
+  a->use_graph = n->use_graph;
+  cup2d_amr_destroy(n); // the old mesh: plan, fields, tables, Poisson context, shapes, the graphs of enqueued steps
+  return CUP2D_OK;
+}
 
 } // namespace cup2d
 
@@ -214,80 +549,130 @@ int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level
   }
   for (int64_t k = 0; k < nold; k++)
     if (used[k] != 1) return reject("old block " + std::to_string(k) + (used[k] ? " is used twice" : " is not covered"));
-  // the new context (plan = 2:1 check, zeroed fields, cell sizes, coarse faces); the old one stays valid until the swap
-  cup2d_amr *n = nullptr;
-  int rc = cup2d_amr_create(nblocks_new, new_level_ij, bpdx, bpdy, a->h0, a->nu, a->device, &n);
-  if (rc) return rc;
-  auto fail = [&](int code) {
-    cup2d_amr_destroy(n);
-    return code;
-  };
-  // lab rows of the refined parents on the old mesh (kind 4: vector, 5: scalar)
-  std::vector<int64_t> rp[2];
-  std::vector<int32_t> sb[2], sc[2];
-  std::vector<double> w[2];
-  for (int k = 0; k < 2; k++)
-    if ((rc = amr_plan_subset_rows(a->plan, 4 + k, (int64_t)parents.size(), parents.data(), rp[k], sb[k], sc[k], w[k]))) return fail(rc);
-  const int fields[RG_NF] = {CUP2D_TMP, CUP2D_CHI, CUP2D_VEL, CUP2D_VOLD, CUP2D_PRES, CUP2D_POLD};
-  RgFields F;
-  F.off2[0] = 0;
-  for (int f = 0; f < RG_NF; f++) {
-    F.src[f] = a->f[fields[f]], F.dst[f] = n->f[fields[f]], F.dim[f] = dim_of(fields[f]);
-    F.off2[f + 1] = F.off2[f] + 32 * F.dim[f];
-  }
-  std::vector<void *> tmp;
-  auto up = [&](const auto &h, auto **d) -> bool {
-    using T = typename std::remove_reference<decltype(h[0])>::type;
-    if (cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T)) != cudaSuccess) return false;
-    tmp.push_back((void *)*d);
-    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
-  };
-  auto release = [&] {
-    for (void *p : tmp) cudaFree(p);
-  };
-  int2 *d_pairs = nullptr;
-  int4 *d_kids = nullptr;
-  int *d_cdst = nullptr, *d_child = nullptr;
-  RgLab L = {};
-  bool ok = up(pairs, &d_pairs) && up(kids, &d_kids) && up(cdst, &d_cdst) && up(child_dst, &d_child);
-  for (int k = 0; k < 2 && ok; k++) {
-    int64_t *r = nullptr;
-    int *b = nullptr, *c = nullptr;
-    double *ww = nullptr;
-    ok = up(rp[k], &r) && up(sb[k], &b) && up(sc[k], &c) && up(w[k], &ww);
-    L.rowptr[k] = r, L.sb[k] = b, L.sc[k] = c, L.w[k] = ww;
-  }
-  L.rbeg[0] = 0;
-  for (int f = 0; f < RG_NF; f++) L.rbeg[f + 1] = L.rbeg[f] + (int64_t)rp[F.dim[f] == 2 ? 0 : 1].size() - 1;
-  for (int f = 0; f < RG_NF && ok; f++) {
-    ok = cudaMalloc(&L.lab[f], std::max<size_t>((size_t)parents.size() * 100 * F.dim[f], 1) * sizeof(double)) == cudaSuccess;
-    if (ok) tmp.push_back(L.lab[f]);
-  }
-  if (!ok) {
-    release();
+  RgScratch S;
+  const int2 *d_pairs = S.up(pairs);
+  const int4 *d_kids = S.up(kids);
+  const int *d_cdst = S.up(cdst), *d_child = S.up(child_dst);
+  if (!S.ok) {
     set_error("cup2d_amr_regrid: out of device memory");
-    return fail(CUP2D_ECUDA);
+    return CUP2D_ECUDA;
   }
-  const int64_t np = (int64_t)pairs.size(), ng = (int64_t)kids.size(), nq = (int64_t)parents.size();
-  if (np) amr_regrid_copy_kernel<<<rg_grid(np * F.off2[RG_NF]), 256, 0, a->stream>>>(F, d_pairs, np);
-  if (ng) amr_regrid_compress_kernel<<<rg_grid(ng * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, d_cdst, d_kids, ng);
-  if (nq) {
-    amr_regrid_lab_kernel<<<rg_grid(L.rbeg[RG_NF]), 256, 0, a->stream>>>(F, L);
-    amr_regrid_refine_kernel<<<rg_grid(nq * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, L, d_child, nq);
+  return regrid_apply(a, "cup2d_amr_regrid", nblocks_new, new_level_ij, bpdx, bpdy, parents, d_pairs, (int64_t)pairs.size(),
+                      d_kids, d_cdst, (int64_t)kids.size(), d_child);
+}
+
+/* adapt() in one call: tagging (block_linf == NULL) or the caller's per-block values, the refine / compress decision and the
+ * order of the new list on the device (bitwise cup2d_amr_adapt_mesh), then the transfer of cup2d_amr_regrid fed from the
+ * device.  Downloaded: the new block list (the host builds its plan) and the refined parents (their lab rows). */
+int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double ctol, int level_max, int64_t *nblocks_out,
+                    int32_t *changed_out) {
+  if (!a || level_max < 1 || level_max > 20) {
+    set_error("cup2d_amr_adapt: bad arguments");
+    return CUP2D_EINVAL;
   }
-  const bool launched = cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(a->stream) == cudaSuccess;
-  release();
-  if (!launched) {
-    set_error("cup2d_amr_regrid: transfer kernels failed");
-    return fail(CUP2D_ECUDA);
+  if (a->dist || a->nranks > 1) {
+    set_error("cup2d_amr_adapt: contexts on several ranks cannot be regridded (blocks would have to migrate between ranks)");
+    return CUP2D_ESTATE;
   }
-  // swap: the handle takes the new mesh's internals; handle, stream, device, h0, nu, the fast flag and the graph switch stay
-  std::swap(*a, *n);
-  std::swap(a->stream, n->stream);
-  a->fast = n->fast;
-  a->use_graph = n->use_graph;
-  cup2d_amr_destroy(n); // the old mesh: plan, fields, tables, Poisson context, shapes, the graphs of enqueued steps
+  int bpdx = 0, bpdy = 0;
+  const std::vector<int> &old = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
+  const int64_t nold = a->nb;
+  if (((int64_t)std::max(bpdx, bpdy) << (level_max - 1)) >= (1 << 29)) {
+    set_error("cup2d_amr_adapt: the finest level has 2^29 blocks or more per direction");
+    return CUP2D_EINVAL;
+  }
+  for (int64_t k = 0; k < nold; k++)
+    if (old[3 * k] >= level_max) {
+      set_error("cup2d_amr_adapt: block " + std::to_string(k) + " is at or above level_max");
+      return CUP2D_EINVAL;
+    }
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  RgScratch S;
+  const double *d_linf = a->d_part;
+  if (block_linf) {
+    d_linf = S.up(std::vector<double>(block_linf, block_linf + nold));
+  } else {
+    const int rc = amr_adapt_tags_enqueue(a, rtol, level_max);
+    if (rc) return rc;
+  }
+  const int64_t npad = pow2_at_least(nold);
+  const CurveTables tables(bpdx, bpdy);
+  const int64_t *d_zsave = S.up(tables.zsave);
+  const int32_t *d_inv = S.up(tables.inv);
+  int *d_lij = S.up(old);
+  u64 *d_key = S.get<u64>(npad);
+  int *d_id = S.get<int>(npad), *st = S.get<int>(nold), *st2 = S.get<int>(nold);
+  int4 *sa = S.get<int4>(nold), *sb = S.get<int4>(nold);
+  if (!S.ok) {
+    set_error("cup2d_amr_adapt: out of device memory");
+    return CUP2D_ECUDA;
+  }
+  cudaStream_t stream = a->stream;
+  const int g = rg_grid(nold);
+  // the old mesh's index, the states, the 2:1 passes level by level, the sibling agreement
+  amr_adapt_index_kernel<<<rg_grid(npad), 256, 0, stream>>>(d_lij, d_key, d_id, nold, npad);
+  bitonic_sort(stream, d_key, d_id, npad);
+  const AdMesh M{d_lij, AdIndex{d_key, d_id, nold}, bpdx, bpdy, level_max, nold};
+  amr_adapt_state_kernel<<<g, 256, 0, stream>>>(M, d_linf, rtol, ctol, st);
+  for (int lv = level_max - 1; lv >= 0; lv--) {
+    amr_adapt_finer_kernel<<<g, 256, 0, stream>>>(M, st, lv);
+    if (lv == 0) break;
+    amr_adapt_same_kernel<<<g, 256, 0, stream>>>(M, st, st2, lv);
+    std::swap(st, st2);
+  }
+  amr_adapt_siblings_kernel<<<g, 256, 0, stream>>>(M, st, st2);
+  std::swap(st, st2);
+  // offsets of every old block's contribution: inclusive scan of the counts (ends in sa)
+  amr_adapt_count_kernel<<<g, 256, 0, stream>>>(M, st, sa);
+  for (int64_t d = 1; d < nold; d <<= 1) {
+    amr_adapt_scan_kernel<<<g, 256, 0, stream>>>(sa, sb, nold, d);
+    std::swap(sa, sb);
+  }
+  int4 tot;
+  CUP2D_CUDA(cudaGetLastError());
+  CUP2D_CUDA(cudaMemcpyAsync(&tot, sa + nold - 1, sizeof(int4), cudaMemcpyDeviceToHost, stream));
+  CUP2D_CUDA(cudaStreamSynchronize(stream));
+  const int64_t nnew = tot.x, np = tot.y, nq = tot.z, ng = tot.w, npad2 = pow2_at_least(nnew);
+  // the new list in emission order, sorted by (Encode, emission index) as the host's std::sort of (key, q) pairs
+  int *out_lij = S.get<int>(3 * nnew), *new_lij = S.get<int>(3 * nnew), *rank = S.get<int>(nnew);
+  int *d_parents = S.get<int>(nq), *d_child = S.get<int>(4 * nq), *d_cdst = S.get<int>(ng);
+  u64 *key2 = S.get<u64>(npad2);
+  int *val2 = S.get<int>(npad2);
+  int2 *d_pairs = S.get<int2>(np);
+  int4 *d_kids = S.get<int4>(ng);
+  if (!S.ok) {
+    set_error("cup2d_amr_adapt: out of device memory");
+    return CUP2D_ECUDA;
+  }
+  amr_adapt_emit_kernel<<<rg_grid(std::max(nold, npad2)), 256, 0, stream>>>(M, st, sa, tables.curve(level_max, d_zsave, d_inv),
+                                                                           out_lij, key2, val2, nnew, npad2, d_parents);
+  bitonic_sort(stream, key2, val2, npad2);
+  amr_adapt_rank_kernel<<<rg_grid(nnew), 256, 0, stream>>>(val2, out_lij, new_lij, rank, nnew);
+  amr_adapt_transfer_kernel<<<g, 256, 0, stream>>>(M, st, sa, rank, d_pairs, d_child, d_kids, d_cdst);
+  CUP2D_CUDA(cudaGetLastError());
+  std::vector<int32_t> nl((size_t)3 * nnew), parents((size_t)nq);
+  CUP2D_CUDA(cudaMemcpyAsync(nl.data(), new_lij, nl.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  if (nq) CUP2D_CUDA(cudaMemcpyAsync(parents.data(), d_parents, parents.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+  CUP2D_CUDA(cudaStreamSynchronize(stream));
+  const bool same = nnew == nold && std::equal(old.begin(), old.end(), nl.begin());
+  const int rc = same ? CUP2D_OK : regrid_apply(a, "cup2d_amr_adapt", nnew, nl.data(), bpdx, bpdy, parents, d_pairs, np, d_kids,
+                                                d_cdst, ng, d_child);
+  if (rc) return rc;
+  if (nblocks_out) *nblocks_out = nnew;
+  if (changed_out) *changed_out = !same;
   return CUP2D_OK;
+}
+
+/* the context's block list [n][3] (level, i, j) into level_ij_out (NULL: only the count) */
+int64_t cup2d_amr_blocks(const cup2d_amr *a, int32_t *level_ij_out) {
+  if (!a) {
+    set_error("cup2d_amr_blocks: bad arguments");
+    return CUP2D_EINVAL;
+  }
+  int bpdx = 0, bpdy = 0;
+  const std::vector<int> &lij = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
+  if (level_ij_out) std::copy(lij.begin(), lij.end(), level_ij_out);
+  return (int64_t)lij.size() / 3;
 }
 
 } // extern "C"

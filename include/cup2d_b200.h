@@ -368,6 +368,18 @@ int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t b
  * again, as ongrid() does after adapt()).  CUP2D_EINVAL, context untouched, for a mesh that is not one step away;
  * CUP2D_ESTATE for contexts on several ranks.  The same block list is a no-op. */
 int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level_ij);
+/* adapt() in one call, decision included (csrc/amr_regrid.cu): block_linf == NULL runs cup2d_amr_adapt_tags on the device
+ * without downloading it (the tagging field is left in tmp as there); otherwise block_linf[nblocks] are the caller's per-block
+ * values (host doubles; any criterion).  The refine / compress decision and the order of the new list are made on the device,
+ * the same list as cup2d_amr_adapt_mesh; then the context is regridded in place as by cup2d_amr_regrid onto that list, with
+ * the same fields.  Only the new block list and the refined parents cross to the host.  An unchanged list is a no-op after
+ * the tagging.  nblocks_out (new block count) and changed_out (0 / 1) may be NULL; cup2d_amr_blocks reads the new list.
+ * CUP2D_EINVAL, context untouched, for level_max outside 1..20 or a block at or above level_max; CUP2D_ESTATE for contexts
+ * on several ranks. */
+int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double ctol, int level_max, int64_t *nblocks_out,
+                    int32_t *changed_out);
+/* the context's block list, [n][3] (level, i, j), into level_ij_out; NULL: only the count n */
+int64_t cup2d_amr_blocks(const cup2d_amr *a, int32_t *level_ij_out);
 
 /* Bodies on a multi-level mesh: the cup2d_shape_* calls (above) on the cup2d_amr context, with the cell size and the block
  * position taken per block (Info::h, Info::origin, main.cpp:695-696).  block_ids index the context's blocks; a shape's
