@@ -316,7 +316,9 @@ class AmrSimulation:
     def ongrid(self, bodies):
         """ongrid()'s rasterisation (main.cpp:4019-4024, 4208-4556) of `bodies` into chi, tmp and the shapes' obstacle blocks.
         A body is a mapping with the nine midline arrays of MIDLINE (shape frame, as at main.cpp:4208), "center", "orientation"
-        and "center_of_mass".  Returns [nshapes, 10]: Mass, COM_x, COM_y, new centre of mass x, y, m, j, u, v, a."""
+        and "center_of_mass".  Returns [nshapes, 10]: Mass, COM_x, COM_y, new centre of mass x, y, m, j, u, v, a.
+        On a distributed context every rank passes the same bodies and gets the same [nshapes, 10] (the sums all-reduced);
+        the shapes' obstacle blocks are this rank's own, numbered locally (0 = the first block of its range)."""
         arrs, structs = [], (_l.Body * len(bodies))()
         for k, b in enumerate(bodies):
             st = structs[k]
@@ -348,7 +350,8 @@ class AmrSimulation:
 
     def shape_get(self, shape, dist=True):
         """shape `shape`'s obstacle blocks on the device: dict of ids [nob], chi [nob,8,8], dist [nob,8,8] (shapes placed by
-        ongrid; None with dist=False) and udef [nob,8,8,2]"""
+        ongrid; None with dist=False) and udef [nob,8,8,2].  On a distributed context: this rank's blocks, ids local (add
+        rank_begin[rank] for the index in the whole list), as shape_set takes them"""
         n = self.lib.cup2d_amr_shape_get(self._h, shape, None, None, None, None)
         if n < 0:
             _l.check(int(n))
@@ -371,7 +374,9 @@ class AmrSimulation:
 
     def collide(self, motions):
         """the collision model (main.cpp:6705-6943) of shapes 0 .. len(motions)-1.  A motion is a mapping with u, v, omega (after
-        the 3x3 solve), center_of_mass, M, J and length.  Returns (uvw [N,3] after the model, sums [N,20] of main.cpp:6814-6837)"""
+        the 3x3 solve), center_of_mass, M, J and length.  Returns (uvw [N,3] after the model, sums [N,20] of main.cpp:6814-6837).
+        On a distributed context every rank passes the same motions: common blocks are found among its own obstacle blocks,
+        the sums all-reduced, and every rank gets the same result"""
         st = (_l.Rigid * len(motions))()
         for k, m in enumerate(motions):
             r = st[k]
@@ -384,14 +389,16 @@ class AmrSimulation:
 
     # ---- surface normals and force diagnostics on the device (cup2d_amr_surface / _surface_get / _forces) ----
     def surface(self, n):
-        """ComputeSurfaceNormals (main.cpp:3774-3828) of shapes 0 .. n-1 on chi and tmp as they stand (after ongrid)"""
+        """ComputeSurfaceNormals (main.cpp:3774-3828) of shapes 0 .. n-1 on chi and tmp as they stand (after ongrid); on a
+        distributed context, of this rank's obstacle blocks (every rank makes the call)"""
         _l.check(self.lib.cup2d_amr_surface(self._h, int(n)))
 
     SKIN = ("x_s", "y_s", "p_s", "u_s", "v_s", "nx_s", "ny_s", "omega_s", "uDef_s", "vDef_s", "fX_s", "fY_s", "fXv_s", "fYv_s")
 
     def surface_get(self, shape):
         """shape `shape`'s surface points: dict of block [n] (block ids), ixy [n, 2], normal [n, 3] = (dchidx, dchidy, D) and
-        skin [n, 14] (the columns of SKIN, of the last forces call; zero before)"""
+        skin [n, 14] (the columns of SKIN, of the last forces call; zero before).  On a distributed context: this rank's
+        points, block ids local as in shape_get"""
         n = self.lib.cup2d_amr_surface_get(self._h, int(shape), None, None, None, None)
         if n < 0:
             _l.check(int(n))
@@ -410,7 +417,8 @@ class AmrSimulation:
     def forces(self, motions):
         """KernelComputeForces and its reductions (main.cpp:5573-5746, 7188-7284) for shapes 0 .. len(motions)-1 from vel,
         pres, chi and each shape's u_def.  A motion is a mapping as for collide (u, v and center_of_mass are read).  Returns
-        [N, 23] with the columns of FORCES"""
+        [N, 23] with the columns of FORCES.  On a distributed context every rank passes the same motions and gets the same
+        [N, 23] (the ranks' sums all-reduced)"""
         st = (_l.Rigid * len(motions))()
         for k, m in enumerate(motions):
             r = st[k]

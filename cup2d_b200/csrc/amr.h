@@ -93,8 +93,15 @@ int amr_ensure_ij(cup2d_amr *a);
 extern "C" int amr_dist_refresh(cup2d_amr *a, int field);
 // distributed contexts: v[0..n) summed over all ranks (identical result everywhere); a no-op otherwise
 extern "C" int amr_dist_sum(cup2d_amr *a, double *v, int n);
+// distributed contexts on several ranks: the host array v[0..n) summed over all ranks in one launch and one host wait, the
+// ranks' values added in rank order, so every rank gets the same bits; CUP2D_ECOMM if the ranks pass different n or a peer
+// never arrives.  A no-op otherwise (one rank included).
+extern "C" int amr_dist_sum_vec(cup2d_amr *a, double *v, int n);
 // fast-kernel tables of a distributed context for its block range [b0, b1): slot_of[global block] = local slot or -1
 int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64_t b0, int64_t b1);
+// distributed contexts: the compact ghost rows of stencil kind `which` (ncell lab entries per block) of the context's own
+// irregular blocks, every source named by its local slot (csrc/amr_fast.cu); CUP2D_EINVAL if a source is not a halo slot
+int amr_ghosts_dist(cup2d_amr *a, int which, int ncell, cup2d::GhostDev &g);
 
 struct cup2d_amr {
   int64_t nb = 0;
@@ -158,6 +165,8 @@ struct cup2d_amr {
   std::vector<Surface> surf;
   double *d_fo_part = nullptr;      // [obstacle blocks][19] per-block accumulators, then [nshapes][19] sums
   size_t fo_part_cap = 0;
+  double *d_vsum = nullptr;         // distributed contexts: the values of amr_dist_sum_vec and its status word
+  size_t vsum_cap = 0;
   // enqueued steps (cup2d_amr_step_enqueue / _pressure_enqueue, csrc/amr_ops.cu): the device record (AMR_REC_*), the events
   // that join the Poisson context's stream to this one, one executable graph per argument set (cudaGraphExec_t / cudaGraph_t)
   double *d_rec = nullptr;

@@ -16,6 +16,8 @@
 // 6863-6943 with collision() / compute_j() restated in the reference's expression order, pairs in (i ascending, j > i
 // ascending) order.  The file is compiled without FMA contraction, device (-fmad=false) and host (-ffp-contract=off) code
 // alike (Makefile), like the reference's host build, so every expression rounds as it does there.
+// On a distributed context (cup2d_amr_create_ranks) the shapes hold the rank's own obstacle blocks, so the common blocks
+// are those of the rank; its 20 N sums are all-reduced (amr_dist_sum_vec, as MPI_Allreduce at 6838) before the pair loop.
 #include "sim.h"
 #include "amr.h"
 #include <algorithm>
@@ -280,8 +282,8 @@ int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *su
     set_error("cup2d_amr_collide: bad arguments (1..64 shapes)");
     return CUP2D_EINVAL;
   }
-  if (a->dist || a->nranks > 1) {
-    set_error("cup2d_amr_collide: contexts on several ranks are not supported");
+  if (!a->dist && a->nranks > 1) {
+    set_error("cup2d_amr_collide: contexts with operators replicated on several ranks (cup2d_amr_set_ranks) are not supported");
     return CUP2D_ESTATE;
   }
   for (int s = 0; s < nshapes; s++) {
@@ -343,6 +345,7 @@ int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *su
   std::vector<double> sums((size_t)nshapes * 20);
   CUP2D_CUDA(cudaMemcpyAsync(sums.data(), a->d_co_sums, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, a->stream));
   CUP2D_CUDA(cudaStreamSynchronize(a->stream));
+  if ((rc = amr_dist_sum_vec(a, sums.data(), 20 * nshapes))) return rc; // the ranks' sums, as MPI_Allreduce (6838)
   co_pairs(nshapes, sums.data(), shapes);
   if (sums20) std::copy(sums.begin(), sums.end(), sums20);
   return CUP2D_OK;

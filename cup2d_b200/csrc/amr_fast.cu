@@ -424,6 +424,62 @@ int amr_pressure_gradient_fast(cup2d_amr *a, double dt, const double *ddt) {
   return CUP2D_OK;
 }
 
+// The compact ghost rows of one stencil kind for a DISTRIBUTED context: the plan's rows of the irregular blocks in this
+// rank's range, renumbered to the rank's irregular list (local position * ncell + lab entry), sources to local slots.
+int amr_ghosts_dist(cup2d_amr *a, int which, int ncell, cup2d::GhostDev &g) {
+  using namespace cup2d;
+  const int64_t b0 = a->gbegin, b1 = a->gbegin + a->nb;
+  const int64_t nirr_g = cup2d_amr_plan_irregular(a->plan, nullptr);
+  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1)), local_of_irr(std::max<int64_t>(nirr_g, 1), -1);
+  cup2d_amr_plan_irregular(a->plan, irr.data());
+  int64_t nirr = 0;
+  for (int64_t qi = 0; qi < nirr_g; qi++)
+    if (irr[qi] >= b0 && irr[qi] < b1) local_of_irr[qi] = (int32_t)nirr++;
+  int64_t nrows_g = 0;
+  const int64_t nnz_g = cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, nullptr, nullptr, nullptr, nullptr, nullptr);
+  if (nnz_g < 0) return CUP2D_EINVAL;
+  std::vector<int64_t> rp_g(nrows_g + 1);
+  std::vector<int32_t> dst_g(std::max<int64_t>(nrows_g, 1)), sb_g(std::max<int64_t>(nnz_g, 1)), sc_g(std::max<int64_t>(nnz_g, 1));
+  std::vector<double> w_g(std::max<int64_t>(nnz_g, 1));
+  cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, rp_g.data(), dst_g.data(), sb_g.data(), sc_g.data(), w_g.data());
+  std::vector<int64_t> rp(1, 0);
+  std::vector<int32_t> dst, sb, sc;
+  std::vector<double> w;
+  for (int64_t row = 0; row < nrows_g; row++) {
+    const int32_t ql = local_of_irr[dst_g[row] / ncell];
+    if (ql < 0) continue;
+    dst.push_back(ql * ncell + dst_g[row] % ncell);
+    for (int64_t e = rp_g[row]; e < rp_g[row + 1]; e++) {
+      const int32_t sl = a->slot_of[sb_g[e]];
+      if (sl < 0) {
+        set_error("distributed context: a lab source lies outside the halo set");
+        return CUP2D_EINVAL;
+      }
+      sb.push_back(sl);
+      sc.push_back(sc_g[e]);
+      w.push_back(w_g[e]);
+    }
+    rp.push_back((int64_t)w.size());
+  }
+  const int64_t nrows = (int64_t)dst.size();
+  std::vector<int64_t> grow(nirr + 1, nrows);
+  for (int64_t row = nrows - 1; row >= 0; row--) grow[dst[row] / ncell] = row;
+  for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]);
+  auto up = [](auto **d, const auto &h) -> cudaError_t {
+    using T = typename std::remove_reference<decltype(h[0])>::type;
+    cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
+    if (e != cudaSuccess) return e;
+    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
+  };
+  CUP2D_CUDA(up(&g.rowptr, rp));
+  CUP2D_CUDA(up(&g.dst, dst));
+  CUP2D_CUDA(up(&g.sb, sb));
+  CUP2D_CUDA(up(&g.sc, sc));
+  CUP2D_CUDA(up(&g.w, w));
+  CUP2D_CUDA(up(&g.grow, grow)); // last: marks the table complete
+  return CUP2D_OK;
+}
+
 // Tables of a DISTRIBUTED context: the plan knows the whole mesh; this rank keeps what concerns its blocks [b0, b1) and
 // names every block by its local slot (own blocks first, then the halo slots of the field arrays): slot_of[global block] or -1.
 int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64_t b0, int64_t b1) {
@@ -450,51 +506,16 @@ int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64
     }
   }
   const int64_t nirr_g = cup2d_amr_plan_irregular(a->plan, nullptr);
-  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1)), irr_of(nloc, -1), local_of_irr(std::max<int64_t>(nirr_g, 1), -1);
+  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1)), irr_of(nloc, -1);
   cup2d_amr_plan_irregular(a->plan, irr.data());
   int64_t nirr = 0;
   for (int64_t qi = 0; qi < nirr_g; qi++)
-    if (irr[qi] >= b0 && irr[qi] < b1) {
-      local_of_irr[qi] = (int32_t)nirr;
-      irr_of[irr[qi] - b0] = (int32_t)nirr++;
-    }
+    if (irr[qi] >= b0 && irr[qi] < b1) irr_of[irr[qi] - b0] = (int32_t)nirr++;
   a->nirr = nirr;
   const int ncell[3] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10};
   for (int which = 0; which < 3; which++) {
-    int64_t nrows_g = 0;
-    const int64_t nnz_g = cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, nullptr, nullptr, nullptr, nullptr, nullptr);
-    if (nnz_g < 0) return CUP2D_EINVAL;
-    std::vector<int64_t> rp_g(nrows_g + 1);
-    std::vector<int32_t> dst_g(std::max<int64_t>(nrows_g, 1)), sb_g(std::max<int64_t>(nnz_g, 1)), sc_g(std::max<int64_t>(nnz_g, 1));
-    std::vector<double> w_g(std::max<int64_t>(nnz_g, 1));
-    cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, rp_g.data(), dst_g.data(), sb_g.data(), sc_g.data(), w_g.data());
-    std::vector<int64_t> rp(1, 0);
-    std::vector<int32_t> dst, sb, sc;
-    std::vector<double> w;
-    for (int64_t row = 0; row < nrows_g; row++) {
-      const int32_t ql = local_of_irr[dst_g[row] / ncell[which]];
-      if (ql < 0) continue;
-      dst.push_back(ql * ncell[which] + dst_g[row] % ncell[which]);
-      for (int64_t e = rp_g[row]; e < rp_g[row + 1]; e++) {
-        const int32_t sl = slot(sb_g[e]);
-        if (sl < 0) return CUP2D_EINVAL;
-        sb.push_back(sl);
-        sc.push_back(sc_g[e]);
-        w.push_back(w_g[e]);
-      }
-      rp.push_back((int64_t)w.size());
-    }
-    const int64_t nrows = (int64_t)dst.size();
-    std::vector<int64_t> grow(nirr + 1, nrows);
-    for (int64_t row = nrows - 1; row >= 0; row--) grow[dst[row] / ncell[which]] = row;
-    for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]);
-    GhostDev &g = a->gt[which];
-    CUP2D_CUDA(up(&g.grow, grow));
-    CUP2D_CUDA(up(&g.rowptr, rp));
-    CUP2D_CUDA(up(&g.dst, dst));
-    CUP2D_CUDA(up(&g.sb, sb));
-    CUP2D_CUDA(up(&g.sc, sc));
-    CUP2D_CUDA(up(&g.w, w));
+    const int rc = amr_ghosts_dist(a, which, ncell[which], a->gt[which]);
+    if (rc) return rc;
   }
   CUP2D_CUDA(up(&a->d_nbr4, n4));
   CUP2D_CUDA(up(&a->d_irr_of, irr_of));

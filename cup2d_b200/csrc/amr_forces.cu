@@ -21,6 +21,9 @@
 //   amr_forces_sum_kernel  per shape, one thread per quantity: the blocks in ascending id order (7210-7231), as the reference's
 //                       shape sums, which on one rank are its MPI_Allreduce of 19.
 //   The four derived quantities (7273-7280) on the host.  One host wait.
+// On a distributed context (cup2d_amr_create_ranks) both calls run on the rank's own obstacle blocks: the fields the labs
+// read are refreshed from their owners first, the tables name blocks by local slot, and the 19 sums per shape are
+// all-reduced (amr_dist_sum_vec, as the reference's MPI_Allreduce at 7252) before the derived quantities.
 // The file is compiled without FMA contraction, device (-fmad=false) and host (-ffp-contract=off) code alike (Makefile), like
 // the reference's host build, so every expression rounds as it does there.
 #include "sim.h"
@@ -322,7 +325,8 @@ static int fo_grow(void **p, size_t *cap, size_t bytes) {
   return CUP2D_OK;
 }
 
-// the force labs' tables, on first use and until a regrid: the 8-neighbour table and the compact ghost rows of kinds 6 and 3
+// the force labs' tables, on first use and until a regrid: the 8-neighbour table and the compact ghost rows of kinds 6 and 3.
+// A distributed context keeps the rows of its own blocks and names every neighbour and source by its local slot.
 static int fo_tables(cup2d_amr *a) {
   int rc = amr_fast_tables(a);
   if (rc) return rc;
@@ -333,9 +337,24 @@ static int fo_tables(cup2d_amr *a) {
     return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
   };
   if (!a->d_nbr8) {
-    std::vector<int32_t> n8((size_t)8 * a->nb);
+    const int64_t nall = a->dist ? a->nglobal : a->nb;
+    std::vector<int32_t> n8((size_t)8 * nall);
     if (cup2d_amr_plan_neighbours(a->plan, n8.data())) return CUP2D_EINVAL;
+    if (a->dist) { // this rank's rows, same-level neighbours by slot (the halo set holds them); walls and level jumps keep their codes
+      n8.erase(n8.begin(), n8.begin() + 8 * a->gbegin);
+      n8.resize((size_t)8 * a->nb);
+      for (auto &g : n8)
+        if (g >= 0 && (g = a->slot_of[g]) < 0) {
+          set_error("distributed context: a lab source lies outside the halo set");
+          return CUP2D_EINVAL;
+        }
+    }
     CUP2D_CUDA(up(&a->d_nbr8, n8));
+  }
+  if (a->dist) {
+    for (int which : {3, 6})
+      if (!a->gt[which].grow && (rc = amr_ghosts_dist(a, which, which == 6 ? 16 * 16 * 2 : 16 * 16, a->gt[which]))) return rc;
+    return CUP2D_OK;
   }
   const int64_t nirr = cup2d_amr_plan_irregular(a->plan, nullptr);
   for (int which : {3, 6}) {
@@ -366,8 +385,8 @@ static int fo_check(cup2d_amr *a, int nshapes, const char *who) {
     set_error(std::string(who) + ": bad arguments (1..64 shapes)");
     return CUP2D_EINVAL;
   }
-  if (a->dist || a->nranks > 1) {
-    set_error(std::string(who) + ": contexts on several ranks are not supported");
+  if (!a->dist && a->nranks > 1) {
+    set_error(std::string(who) + ": contexts with operators replicated on several ranks (cup2d_amr_set_ranks) are not supported");
     return CUP2D_ESTATE;
   }
   for (int s = 0; s < nshapes; s++)
@@ -402,6 +421,8 @@ int cup2d_amr_surface(cup2d_amr *a, int nshapes) {
   if (rc) return rc;
   CUP2D_CUDA(cudaSetDevice(a->device));
   if ((rc = amr_fast_tables(a))) return rc;
+  // the +-1 labs of chi and tmp read the halo slots of a distributed context
+  if ((rc = amr_dist_refresh(a, CUP2D_CHI)) || (rc = amr_dist_refresh(a, CUP2D_TMP))) return rc;
   if (a->surf.size() < a->shapes.size()) a->surf.resize(a->shapes.size());
   for (int s = 0; s < nshapes; s++) { // 64 point slots per obstacle block
     cup2d_amr::Surface &q = a->surf[s];
@@ -494,6 +515,8 @@ int cup2d_amr_forces(cup2d_amr *a, int nshapes, const cup2d_rigid *shapes, doubl
   }
   CUP2D_CUDA(cudaSetDevice(a->device));
   if ((rc = fo_tables(a)) || (rc = amr_ensure_ij(a))) return rc;
+  // the labs of vel and chi read the halo slots of a distributed context; pres is read at the block's own cells only
+  if ((rc = amr_dist_refresh(a, CUP2D_VEL)) || (rc = amr_dist_refresh(a, CUP2D_CHI))) return rc;
   const FoShapes S = fo_shapes(a, nshapes);
   const int total = S.first[nshapes];
   const size_t b_part = ((size_t)total * 19 + (size_t)nshapes * 19) * sizeof(double);
@@ -510,6 +533,7 @@ int cup2d_amr_forces(cup2d_amr *a, int nshapes, const cup2d_rigid *shapes, doubl
   std::vector<double> q19((size_t)nshapes * 19);
   CUP2D_CUDA(cudaMemcpyAsync(q19.data(), d_sums, q19.size() * sizeof(double), cudaMemcpyDeviceToHost, a->stream));
   CUP2D_CUDA(cudaStreamSynchronize(a->stream));
+  if ((rc = amr_dist_sum_vec(a, q19.data(), 19 * nshapes))) return rc; // the ranks' sums, as MPI_Allreduce (7252)
   for (int s = 0; s < nshapes; s++) { // main.cpp:7273-7280
     const double *q = q19.data() + 19 * s;
     double *o = out + 23 * s;

@@ -17,7 +17,10 @@
 //   amr_ongrid_moments_kernel  the seven sums of 4489-4518 per block, cell by cell in order
 //   amr_ongrid_correct_kernel  udef -= (u - a py, v + a px) (4541-4556)
 //   amr_udef_blend_kernel      cup2d_amr_udef_blend: vel = vel (1 - chi) + tmpV chi before the time loop (6566-6575)
-// The host adds the per-block partials in block order (as cup2d_amr_shape_integrals does).  This file is compiled without FMA
+// The host adds the per-block partials in block order (as cup2d_amr_shape_integrals does).  On a distributed context
+// (cup2d_amr_create_ranks) the kernels run over the rank's own blocks, tmp's halo slots are refreshed before the chi kernel
+// (the neighbour table and ghost rows name slots), and the rank's partial sums are all-reduced (amr_dist_sum_vec) before
+// the host uses them, as the reference's MPI_Allreduce at 4483 and 4520.  This file is compiled without FMA
 // contraction (Makefile), like the reference (-O3, no -ffp-contract=fast on x86-64), so every expression rounds as it does there.
 #include "sim.h"
 #include "amr.h"
@@ -469,8 +472,8 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
     set_error("cup2d_amr_ongrid: bad arguments (1..64 bodies and an output array)");
     return CUP2D_EINVAL;
   }
-  if (a->dist || a->nranks > 1) {
-    set_error("cup2d_amr_ongrid: contexts on several ranks are not supported");
+  if (!a->dist && a->nranks > 1) {
+    set_error("cup2d_amr_ongrid: contexts with operators replicated on several ranks (cup2d_amr_set_ranks) are not supported");
     return CUP2D_ESTATE;
   }
   int bpdx = 0, bpdy = 0;
@@ -578,6 +581,7 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
       amr_ongrid_fish_kernel<<<sh.nob, 64, 0, a->stream>>>(S[s], sh.d_ids, ij, a->d_h, a->f[CUP2D_TMP], sh.d_dist, sh.d_X, sh.d_udef);
   }
   CUP2D_CUDA(ev(6));
+  if ((rc = amr_dist_refresh(a, CUP2D_TMP))) return rc; // the +-1 lab of tmp reads the halo slots of a distributed context
   for (int s = 0; s < nshapes; s++) { // Mass / COM partials of every shape, one download
     const cup2d_amr::Shape &sh = a->shapes[s];
     if (sh.nob)
@@ -590,10 +594,13 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
   std::vector<double> hp((size_t)std::max<int64_t>(ntot, 1) * 7);
   CUP2D_CUDA(cudaMemcpyAsync(hp.data(), a->d_og_part, (size_t)ntot * 3 * sizeof(double), cudaMemcpyDeviceToHost, a->stream));
   CUP2D_CUDA(cudaStreamSynchronize(a->stream));
+  std::vector<double> sums((size_t)nshapes * 7, 0.0);
+  for (int s = 0; s < nshapes; s++) // block order (main.cpp:4476-4482)
+    for (int64_t k = pofs[s]; k < pofs[s + 1]; k++)
+      for (int q = 0; q < 3; q++) sums[(size_t)s * 3 + q] += hp[(size_t)k * 3 + q];
+  if ((rc = amr_dist_sum_vec(a, sums.data(), 3 * nshapes))) return rc; // the ranks' partials, as MPI_Allreduce (4483)
   for (int s = 0; s < nshapes; s++) {
-    double com[3] = {0, 0, 0};
-    for (int64_t k = pofs[s]; k < pofs[s + 1]; k++) // block order (main.cpp:4476-4482)
-      for (int q = 0; q < 3; q++) com[q] += hp[(size_t)k * 3 + q];
+    const double *com = sums.data() + (size_t)s * 3;
     double *o = out + 10 * s;
     o[0] = com[0], o[1] = com[1], o[2] = com[2];
     o[3] = bodies[s].center_of_mass[0] + com[1] / com[0]; // main.cpp:4485-4486
@@ -611,11 +618,14 @@ int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double
   CUP2D_CUDA(cudaMemcpyAsync(hp.data(), a->d_og_part, (size_t)ntot * 7 * sizeof(double), cudaMemcpyDeviceToHost, a->stream));
   CUP2D_CUDA(cudaStreamSynchronize(a->stream));
   CUP2D_CUDA(ev(10));
+  std::fill(sums.begin(), sums.end(), 0.0);
+  for (int s = 0; s < nshapes; s++)
+    for (int64_t k = pofs[s]; k < pofs[s + 1]; k++)
+      for (int q = 0; q < 7; q++) sums[(size_t)s * 7 + q] += hp[(size_t)k * 7 + q];
+  if ((rc = amr_dist_sum_vec(a, sums.data(), 7 * nshapes))) return rc; // as MPI_Allreduce (4520)
   for (int s = 0; s < nshapes; s++) {
     const cup2d_amr::Shape &sh = a->shapes[s];
-    double q7[7] = {0, 0, 0, 0, 0, 0, 0};
-    for (int64_t k = pofs[s]; k < pofs[s + 1]; k++)
-      for (int q = 0; q < 7; q++) q7[q] += hp[(size_t)k * 7 + q];
+    const double *q7 = sums.data() + (size_t)s * 7;
     const double m = q7[2], j = q7[3], u = q7[4] / m, v = q7[5] / m, av = q7[6] / j; // main.cpp:4529-4531
     double *o = out + 10 * s;
     o[5] = m, o[6] = j, o[7] = u, o[8] = v, o[9] = av;

@@ -438,7 +438,7 @@ void cup2d_amr_destroy(cup2d_amr *a) {
   }
   for (auto p : a->lab) cudaFree(p);
   cudaFree(a->lab_udef); cudaFree(a->d_h); cudaFree(a->d_cf[0]); cudaFree(a->d_cf[1]); cudaFree(a->d_part);
-  cudaFree(a->d_nbr4); cudaFree(a->d_nbr8); cudaFree(a->d_irr_of); cudaFree(a->d_faceflux);
+  cudaFree(a->d_nbr4); cudaFree(a->d_nbr8); cudaFree(a->d_irr_of); cudaFree(a->d_faceflux); cudaFree(a->d_vsum);
   a->free_shapes();
   for (auto &g : a->gt) {
     cudaFree(g.grow); cudaFree(g.rowptr); cudaFree(g.dst); cudaFree(g.sb); cudaFree(g.sc); cudaFree(g.w);
@@ -609,10 +609,64 @@ int amr_dist_sum(cup2d_amr *a, double *v, int n) {
   }
   return CUP2D_OK;
 }
+
+// v[0..n) summed over all ranks by one warp, seven values per peer all-reduce; v[n] = 0, or 1 if the ranks disagree on n.
+// n goes round first (its sum and its maximum): every rank sees the same pair, so either all ranks add the values or all
+// of them skip them, and a call made with different arguments on different ranks fails everywhere instead of mixing values.
+constexpr int AMR_VSUM_CHUNK = 7;
+__global__ void __launch_bounds__(32) amr_allreduce_vec_kernel(double *v, int n, Comm comm) {
+  const int lane = threadIdx.x & 31;
+  double cnt[1] = {(double)n}, cmax = (double)n;
+  peer_allreduce<1>(comm, cnt, cmax, lane);
+  if (cnt[0] != comm.nranks * cmax) {
+    if (lane == 0) v[n] = 1.0;
+    return;
+  }
+  for (int k0 = 0; k0 < n; k0 += AMR_VSUM_CHUNK) {
+    double t[AMR_VSUM_CHUNK], m = 0.0;
+#pragma unroll
+    for (int q = 0; q < AMR_VSUM_CHUNK; q++) t[q] = k0 + q < n ? v[k0 + q] : 0.0;
+    __syncwarp();
+    peer_allreduce<AMR_VSUM_CHUNK>(comm, t, m, lane);
+    if (lane == 0)
+      for (int q = 0; q < AMR_VSUM_CHUNK && k0 + q < n; q++) v[k0 + q] = t[q];
+    __syncwarp();
+  }
+  if (lane == 0) v[n] = 0.0;
+}
+int amr_dist_sum_vec(cup2d_amr *a, double *v, int n) {
+  if (!a->dist || a->nranks == 1) return CUP2D_OK;
+  if (!a->poisson->peers_attached) {
+    set_error("distributed context: all-reduce before cup2d_amr_peer_attach");
+    return CUP2D_ESTATE;
+  }
+  const size_t bytes = ((size_t)n + 1) * sizeof(double);
+  if (bytes > a->vsum_cap) {
+    cudaFree(a->d_vsum);
+    a->d_vsum = nullptr, a->vsum_cap = 0;
+    CUP2D_CUDA(cudaMalloc(&a->d_vsum, bytes));
+    a->vsum_cap = bytes;
+  }
+  std::vector<double> h(n + 1);
+  CUP2D_CUDA(cudaMemcpyAsync(a->d_vsum, v, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, a->stream));
+  amr_allreduce_vec_kernel<<<1, 32, 0, a->stream>>>(a->d_vsum, n, a->poisson->comm);
+  CUP2D_CUDA(cudaGetLastError());
+  CUP2D_CUDA(cudaMemcpyAsync(h.data(), a->d_vsum, bytes, cudaMemcpyDeviceToHost, a->stream));
+  CUP2D_CUDA(cudaStreamSynchronize(a->stream));
+  int rc = comm_check(a->poisson);
+  if (rc) return rc;
+  if (h[n] != 0.0) {
+    set_error("distributed context: the ranks summed different numbers of values (the same call with different arguments)");
+    return CUP2D_ECOMM;
+  }
+  std::copy(h.begin(), h.begin() + n, v);
+  return CUP2D_OK;
+}
 #else
 static int dist_allreduce(cup2d_amr *, double &, double &, double &) { return CUP2D_OK; }
 int amr_dist_refresh(cup2d_amr *, int) { return CUP2D_OK; }
 int amr_dist_sum(cup2d_amr *, double *, int) { return CUP2D_OK; }
+int amr_dist_sum_vec(cup2d_amr *, double *, int) { return CUP2D_OK; }
 #endif
 
 /* main.cpp:6579-6595 with h = the smallest cell size of the mesh */
@@ -762,8 +816,10 @@ int cup2d_amr_create_ranks(int64_t nblocks, const int32_t *level_ij, int32_t bpd
   const int64_t nirr_g = cup2d_amr_plan_irregular(plan, nullptr);
   std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1));
   cup2d_amr_plan_irregular(plan, irr.data());
-  const int ncell[4] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10, 16 * 16}; // (3: the chi lab of the tagging rule)
-  for (int which = 0; which < 4; which++) {
+  // kinds 0-3 and 6 (3: the chi lab of the tagging rule and of the forces, 6: the forces' velocity lab)
+  const int kinds[5] = {0, 1, 2, 3, 6}, ncells[5] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10, 16 * 16, 16 * 16 * 2};
+  for (int kk = 0; kk < 5; kk++) {
+    const int which = kinds[kk], ncell = ncells[kk];
     int64_t nrows = 0;
     const int64_t nnz = cup2d_amr_plan_ghosts(plan, which, &nrows, nullptr, nullptr, nullptr, nullptr, nullptr);
     if (nnz < 0) return fail(CUP2D_EINVAL);
@@ -772,7 +828,7 @@ int cup2d_amr_create_ranks(int64_t nblocks, const int32_t *level_ij, int32_t bpd
     std::vector<double> w(std::max<int64_t>(nnz, 1));
     cup2d_amr_plan_ghosts(plan, which, &nrows, rp.data(), dst.data(), sb.data(), sc.data(), w.data());
     for (int64_t row = 0; row < nrows; row++) {
-      const int32_t blk = irr[dst[row] / ncell[which]];
+      const int32_t blk = irr[dst[row] / ncell];
       if (blk < b0 || blk >= b1) continue;
       for (int64_t e = rp[row]; e < rp[row + 1]; e++) extra.push_back(sb[e]);
     }

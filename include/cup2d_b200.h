@@ -413,10 +413,16 @@ typedef struct {
  * for cup2d_amr_shape_integrals / _penalize / _udef_assemble; shapes k >= nshapes are dropped.  dist, tmp and u_def before the
  * correction are bit-identical to the reference; chi on blocks whose +-1 lab needs the ghost tables, and the sums, to rounding.
  * CUP2D_EINVAL (context untouched) for a body with nm < 9 or (nm-1) not a multiple of (nm-1)/8, a missing array or its center outside the domain (the reference
- * aborts, 4009-4013); CUP2D_ESTATE for contexts on several ranks.  1 <= nshapes <= 64. */
+ * aborts, 4009-4013); CUP2D_ESTATE for contexts of cup2d_amr_set_ranks (operators replicated on several ranks).
+ * 1 <= nshapes <= 64.
+ * On a distributed context (cup2d_amr_create_ranks, one rank included) every rank makes the call with the same arguments
+ * and works on its own blocks; the sums are the ranks' partials added across ranks (to rounding of the one-rank result),
+ * identical on every rank; CUP2D_ECOMM if the ranks pass different nshapes or a peer never arrives.  There a shape's obstacle blocks are the rank's own
+ * (possibly none), numbered by their position in the rank's block range, as cup2d_amr_shape_set takes them. */
 int cup2d_amr_ongrid(cup2d_amr *a, int nshapes, const cup2d_body *bodies, double *out);
 /* download shape k's obstacle blocks (any pointer may be NULL; returns nob): ids[nob], chi[nob][64], dist[nob][64] (shapes placed
- * by cup2d_amr_ongrid or given by cup2d_amr_shape_set_dist), udef[nob][64][2] — what the host's forces and skins read */
+ * by cup2d_amr_ongrid or given by cup2d_amr_shape_set_dist), udef[nob][64][2] — what the host's forces and skins read.  On a
+ * distributed context: this rank's obstacle blocks, ids local (rank_begin[rank] + id is the block's index in the whole list) */
 int cup2d_amr_shape_get(cup2d_amr *a, int shape, int32_t *ids, double *chi, double *dist, double *udef);
 /* CUDA-event timing of cup2d_amr_ongrid on the context's stream: timing(a, 1) creates the events and times every following call
  * (0 stops; a regrid clears it); times(a, ms8) gives the last timed call's milliseconds: {whole call on the stream (upload,
@@ -443,8 +449,11 @@ typedef struct {
  * shapes and several simultaneous collisions the reference's parallel loop has no defined order, and neither has its result.
  * sums20 (may be NULL) gets [nshapes][20] in the layout of 6814-6837 (the Z slots zero).  Fields and shape data are not
  * changed.  CUP2D_EINVAL for nshapes outside 1..64, a shape not set or one whose block ids are not strictly ascending
- * (cup2d_amr_ongrid leaves them ascending); CUP2D_ESTATE for a shape without dist or a context on several ranks.  On any
- * error `shapes` and the context are untouched. */
+ * (cup2d_amr_ongrid leaves them ascending); CUP2D_ESTATE for a shape without dist or a context of cup2d_amr_set_ranks.  On
+ * any error `shapes` and the context are untouched.
+ * On a distributed context (cup2d_amr_create_ranks, one rank included) every rank makes the call with the same arguments
+ * and works on its own blocks; the sums are the ranks' partials added across ranks (to rounding of the one-rank result),
+ * identical on every rank; CUP2D_ECOMM if the ranks pass different nshapes or a peer never arrives.  The pair loop then runs on every rank on the same sums. */
 int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *sums20);
 
 /* Surface normals and force diagnostics on a multi-level mesh (csrc/amr_forces.cu), on the obstacle blocks the device holds:
@@ -456,11 +465,13 @@ int cup2d_amr_collide(cup2d_amr *a, int nshapes, cup2d_rigid *shapes, double *su
  * reads its lab rows there without their offset, so three cells per block read a corner ghost no rule writes; those hold
  * chi = 0 and tmp = -1, the reference's values while the bodies are away from the domain walls.  cup2d_amr_shape_set,
  * cup2d_amr_ongrid and cup2d_amr_regrid drop the points.  CUP2D_EINVAL for nshapes outside 1..64 or a shape not set;
- * CUP2D_ESTATE for contexts on several ranks. */
+ * CUP2D_ESTATE for contexts of cup2d_amr_set_ranks.  On a distributed context every rank makes the call: the points of its
+ * own obstacle blocks, the labs' remote blocks refreshed from their owners first. */
 int cup2d_amr_surface(cup2d_amr *a, int nshapes);
 /* shape k's surface points: block[n] (block id), ixy[n][2], normal[n][3] = {dchidx, dchidy, D}; skin[n][14] = x_s, y_s, p_s,
  * u_s, v_s, nx_s, ny_s, omega_s, uDef_s, vDef_s, fX_s, fY_s, fXv_s, fYv_s of the last cup2d_amr_forces call (zero before).
- * Any pointer may be NULL; returns n (CUP2D_EINVAL: no such shape, CUP2D_ESTATE: no points since the shape was last set). */
+ * Any pointer may be NULL; returns n (CUP2D_EINVAL: no such shape, CUP2D_ESTATE: no points since the shape was last set).
+ * On a distributed context: this rank's points, block ids local as in cup2d_amr_shape_get. */
 int64_t cup2d_amr_surface_get(cup2d_amr *a, int shape, int32_t *block, int32_t *ixy, double *normal, double *skin);
 /* KernelComputeForces + main.cpp:7188-7284 from vel, pres, chi and each shape's u_def: out[23*k ..] = quantities[0..18] in the
  * order of 7233-7251 (circulation, perimeter, forcex, forcex_P, forcex_V, torque_P, drag, lift, Pout, PoutNew, PoutBnd, torque,
@@ -468,7 +479,11 @@ int64_t cup2d_amr_surface_get(cup2d_amr *a, int shape, int32_t *block, int32_t *
  * Reads u, v and center_of_mass of shapes[k] (cup2d_rigid, as cup2d_amr_collide leaves them).  Points, then blocks in
  * ascending id order, are added as the reference's serial chains.  Fields and shape data are not changed.  CUP2D_EINVAL for
  * nshapes outside 1..64, a shape not set or a NULL shapes / out; CUP2D_ESTATE for a shape whose surface points were dropped
- * or a context on several ranks.  On any error the context and out are untouched. */
+ * or a context of cup2d_amr_set_ranks.  On any error but CUP2D_ECOMM the context and out are untouched.
+ * On a distributed context (cup2d_amr_create_ranks, one rank included) every rank makes the call with the same arguments
+ * and works on its own blocks; the sums are the ranks' partials added across ranks (to rounding of the one-rank result),
+ * identical on every rank; CUP2D_ECOMM if the ranks pass different nshapes or a peer never arrives.  Pthrust, Pdrag and the efficiencies follow
+ * from the all-reduced sums on every rank. */
 int cup2d_amr_forces(cup2d_amr *a, int nshapes, const cup2d_rigid *shapes, double *out);
 
 #ifdef __cplusplus
