@@ -467,7 +467,7 @@ k_final(double *x0, double *x1, double *x2, const double *__restrict__ zp, const
 // (kp, knu) and (kz, kzr) by the parity of the iteration count (k_init zeroes the first pair), which one captured iteration
 // body of the graph WHILE node serves for every pass.
 #ifndef KTILE_CTAS
-#define KTILE_CTAS 2 // resident CTAs/SM the three kernels are register-bounded for (126-128 registers; at 3 (80) all of them spill)
+#define KTILE_CTAS 2 // resident CTAs/SM k_p_spmv and k_x_final are register-bounded for (128 registers; at 3 (80) both spill)
 #endif
 constexpr int PST = 34; // tile plane row stride in doubles: 16-byte rows, conflict-free 128-bit row reads of a warp
 
@@ -484,6 +484,25 @@ __device__ __forceinline__ void blocks_st(double *__restrict__ f, const int (&sl
 #pragma unroll
   for (int j = 0; j < 4; j++)
     if (sl[j] >= 0) reinterpret_cast<double2 *>(f + (size_t)sl[j] * 64)[lane] = c[j];
+}
+
+// A load that stays in flight while the tile is computed: 16-byte cp.async (SASS LDGSTS) of each lane's pieces of the
+// warp's four blocks into a per-warp stage in shared memory (128 double2, [block][lane]), no registers held meanwhile.  A
+// lane reads back only what it copied itself, so cp.async.wait_all is all the data needs; the caller rewrites a stage
+// only after a CTA barrier that follows the stage's last read.
+__device__ __forceinline__ void stage_ld16(void *smem_dst, const void *gmem_src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void stage_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+__device__ __forceinline__ void blocks_stage(double2 *stg, const double *f, const int (&sl)[4], int lane) {
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+    if (sl[j] >= 0) stage_ld16(stg + j * 32 + lane, f + (size_t)sl[j] * 64 + 2 * lane);
+}
+// after stage_wait(): the chunk layout blocks_ld would have loaded
+__device__ __forceinline__ void blocks_unstage(const double2 *stg, const int (&sl)[4], int lane, double2 (&c)[4]) {
+#pragma unroll
+  for (int j = 0; j < 4; j++) c[j] = sl[j] >= 0 ? stg[j * 32 + lane] : make_double2(0.0, 0.0);
 }
 
 // Shared memory of a tile: z of the 16 interior blocks (plane rows 1..32), row 7 of the S ring blocks (plane row 0),
@@ -562,11 +581,18 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
   double *__restrict__ pn = in ? p0 : p1;
   double *__restrict__ nun = in ? nu0 : nu1;
   double sums[2] = {0, 0};
+  // r^ of the interior blocks is needed only after the preconditioner: it is copied into a stage when the tile starts, so
+  // its load overlaps the preconditioner and the stencil.  Two stages, alternating by tile: a copy is issued only after the
+  // CTA barriers of the tile that read the stage last.
+  __shared__ __align__(16) double2 s_rhat[2 * 4 * 128];
+  int par = 0;
   TILE_LOOP() {
     const int *ts = tiles + (size_t)tile * TILE_SLOTS;
     int sl[4];
 #pragma unroll
     for (int j = 0; j < 4; j++) sl[j] = ts[4 * warp + j];
+    double2 *stg = s_rhat + (par * 4 + (warp & 3)) * 128;
+    if (warp < 4 && !restart) blocks_stage(stg, rhat, sl, lane);
     double2 cp[4], cr[4], ch[4];
     blocks_ld(r, sl, lane, cr);
     if (restart) {
@@ -589,7 +615,10 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
     double2 ca[4];
     tile_precond_lap(v, s_tile, sw, lane, warp, ts, ca);
     if (warp < 4) {
-      if (!restart) blocks_ld(rhat, sl, lane, ch); // loaded late: held across the preconditioner it costs spills
+      if (!restart) { // held in registers across the preconditioner it would cost spills
+        stage_wait();
+        blocks_unstage(stg, sl, lane, ch);
+      }
 #pragma unroll
       for (int j = 0; j < 4; j++) {
         sums[0] = fma(ca[j].x, ch[j].x, sums[0]);
@@ -597,6 +626,7 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
       }
       blocks_st(nun, sl, lane, ca);
     }
+    par ^= 1;
   }
   grid_reduce<2, NT>(sums, 0.0, partials, counter, comm, [=](const double *t, double) {
     st->rhat_nu = t[0];
@@ -605,8 +635,14 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
   });
 }
 
+#ifndef KR_CTAS
+// k_r_spmv holds fewer values than the other two: bounded for 3 CTAs/SM it needs 80 registers and spills 48 bytes, and is
+// still faster than at 2 (more warps to cover its loads).  It launches one wave of its own, so its dot products are
+// partitioned over other CTAs than k_p_spmv's.
+#define KR_CTAS 3
+#endif
 // ---- KB: r' = r - alpha nu' ; t = A M r' ; t.r', t.t -> omega   (cuda.cu:499-518) -------------------------------------
-__global__ void __launch_bounds__(NT, KTILE_CTAS)
+__global__ void __launch_bounds__(NT, KR_CTAS)
 k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, double *__restrict__ t,
          const int *__restrict__ tiles, int ntiles, KrylovState *st, double *partials, unsigned int *counter, Comm comm) {
   if (st->done) return;
@@ -763,7 +799,7 @@ int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream) {
   if (!multi && !has_irr && !s->poisson_only) {
     // one wave of tile CTAs: the tiles in flight then form one compact region of the Hilbert order, whose ring blocks
     // are mostly read from L2
-    const int tgrid = std::min(grid, s->num_sms * KTILE_CTAS);
+    const int tgrid = std::min(grid, s->num_sms * KTILE_CTAS), rgrid = std::min(grid, s->num_sms * KR_CTAS);
     for (int k = 0; k < n; k++) {
       {
         ProfScope prof(s, KC_P_SPMV);
@@ -772,7 +808,7 @@ int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream) {
       }
       {
         ProfScope prof(s, KC_R_SPMV);
-        k_r_spmv<<<tgrid, NT, 0, stream>>>(s->kr, s->knu, s->kzr, s->kt, s->d_tiles, s->ntiles, s->d_state, s->d_partials,
+        k_r_spmv<<<rgrid, NT, 0, stream>>>(s->kr, s->knu, s->kzr, s->kt, s->d_tiles, s->ntiles, s->d_state, s->d_partials,
                                            s->d_counter, s->comm);
       }
       {
