@@ -14,7 +14,7 @@
 //     (set_alpha/beta/omega/rho, cuda.cu:303-330) run in the last CTA of the producing kernel, the
 //     x_opt snapshot (cuda.cu:537) is a rotation among three x buffers, and convergence is a device
 //     flag that turns the remaining launches into no-ops.
-// (On one rank with a uniform grid the five kernels become three, 136 B/cell: see k_p_spmv below.)
+// (On one rank with a uniform grid the five kernels become three, 120 B/cell: see k_p_spmv below.)
 // Traffic per iteration: 23 doubles/cell = 184 B/cell (SURVEY.md §8(d) budgets 25 = 200 B): the half-step update
 // x' = x + alpha z of cuda.cu:498 is deferred into the final kernel, which applies x'' = (x + alpha z_p) + omega z_r
 // in the reference's order (bitwise the same iterate), so the middle kernel neither reads nor writes x or z_p.
@@ -229,19 +229,19 @@ __device__ __forceinline__ void set_loop_condition(unsigned long long handle, co
   double *sw = s_scr + warp * SCR1;                                                               \
   for (int row0 = (blockIdx.x * WPB + warp) * 32; row0 < nrows; row0 += gridDim.x * WPB * 32)
 
-// ---- K0: r = b - A x0 ; rhat = r ; p = nu = 0 ; x[0] = x0 ; err0, |r|^2, sum(x0) -----------------
+// ---- K0: r = b - A x0 ; rhat = r ; x[0] = x0 ; err0, |r|^2, sum(x0) -----------------
+// p = nu = 0 is not stored: the first p-update of a solve (iter 0) takes p = r, which is beta*(0 - omega*0) + r.
 template <bool IRR>
 __global__ void __launch_bounds__(NT)
 k_init(const double *__restrict__ b, const double *__restrict__ x0, double *__restrict__ x,
-       double *__restrict__ r, double *__restrict__ rhat, double *__restrict__ p,
-       double *__restrict__ nu, const int4 *__restrict__ nbr, int nrows, KrylovState *st,
+       double *__restrict__ r, double *__restrict__ rhat, const int4 *__restrict__ nbr, int nrows, KrylovState *st,
        double *partials, unsigned int *counter, Comm comm, IrrView irr, unsigned long long loop_handle) {
   __shared__ __align__(16) double s_scr[WPB * SCR1];
   double sums[2] = {0, 0}; // |r|^2, sum x0
   double mx = 0;
   CHUNK_LOOP() {
     const int nv = min(32, nrows - row0);
-    double xx[8], ax[8], bb[8], zero[8];
+    double xx[8], ax[8], bb[8];
     double2 cx0[4], cb[4];
     chunk_ld(x0, row0, nv, lane, cx0);
     chunk_ld(b, row0, nv, lane, cb);
@@ -253,13 +253,10 @@ k_init(const double *__restrict__ b, const double *__restrict__ x0, double *__re
       sums[0] = fma(bb[i], bb[i], sums[0]);
       sums[1] += xx[i];
       mx = fmax(mx, fabs(bb[i]));
-      zero[i] = 0.0;
     }
     rows_store1(r, row0, nv, sw, lane, bb);
     rows_store1(rhat, row0, nv, sw, lane, bb);
     rows_store1(x, row0, nv, sw, lane, xx);
-    rows_store1(p, row0, nv, sw, lane, zero);
-    rows_store1(nu, row0, nv, sw, lane, zero);
   }
   grid_reduce<2, NT>(sums, mx, partials, counter, comm, [=](const double *t, double m) {
     st->err = st->err_init = st->err_opt = m; // cuda.cu:428-430
@@ -281,14 +278,14 @@ k_pupdate(const double *__restrict__ r, double *__restrict__ rhat, double *__res
   __shared__ __align__(16) double s_scr[WPB * SCR1];
   if (st->done) return;
   const double beta = st->beta, nomega = -st->omega;
-  const bool restart = st->restart_now != 0;
+  const bool restart = st->restart_now != 0, first = st->iter == 0;
   CHUNK_LOOP() {
     const int nv = min(32, nrows - row0);
     // element-wise part in chunk layout (coalesced, no shared memory)
     double2 cp[4], cr[4];
     chunk_ld(r, row0, nv, lane, cr);
-    if (restart) {
-      chunk_st(rhat, row0, nv, lane, cr);
+    if (restart || first) { // p = r: p = nu = 0 at the start of a solve and after a restart (k_init stores neither)
+      if (restart) chunk_st(rhat, row0, nv, lane, cr);
 #pragma unroll
       for (int j = 0; j < 4; j++) cp[j] = cr[j];
     } else {
@@ -456,16 +453,19 @@ k_final(double *x0, double *x1, double *x2, const double *__restrict__ zp, const
 
 // ==== single-rank uniform grids: the same iteration in three kernels that recompute z = M p and z_r = M r ================
 // M is block-local (about 19 FP64 operations per cell), so recomputing it is cheaper than writing z and reading it back:
-// the iteration moves 17 doubles per cell instead of 23.  What stands in the way is the SpMV after each preconditioner: it
-// needs z on the face-neighbour blocks, and z there depends on the whole neighbour block.  So the two SpMV kernels work on
-// the advect stage's tiles (4x4 blocks + their 16 ring blocks) and precondition the ring blocks themselves:
+// the iteration moves 15 doubles per cell instead of 23.  What stands in the way is the SpMV after each preconditioner: it
+// needs z on the face-neighbour blocks, and z there depends on the whole neighbour block.  So the kernels work on the
+// advect stage's tiles (4x4 blocks + their 16 ring blocks) and precondition the ring blocks themselves:
 //   k_p_spmv  (KA): p' = r + beta (p - omega nu) ; z = M p' on tile + ring ; nu' = A z ; rhat.nu' -> alpha      r p nu rhat | p' nu'
-//   k_r_spmv  (KB): r' = r - alpha nu' ; z_r = M r' on tile + ring ; t = A z_r ; t.r', t.t -> omega               r nu'       | t
-//   k_x_final (KC): r' again ; z_p, z_r block-locally ; x = (x + alpha z_p) + omega z_r ; r = r' - omega t ; sums  x p' r nu' t rhat | x r
-// Every element-wise value is computed by the same expression as in the five-kernel path above; only the partition of the
-// dot products differs.  KA reads p and nu of ring blocks, so it must not write them in place: (p, nu) alternate between
-// (kp, knu) and (kz, kzr) by the parity of the iteration count (k_init zeroes the first pair), which one captured iteration
-// body of the graph WHILE node serves for every pass.
+//   k_r_spmv  (KB): r' = r - alpha nu' ; z_r = M r' on tile + ring ; t = A z_r ; t.r', t.t -> omega               r nu'       | r'
+//   k_x_final (KC): z_r = M r' on tile + ring ; t = A z_r ; z_p = M p' ; x = (x + alpha z_p) + omega z_r ;
+//                   r = r' - omega t ; rhat.r, |r|^2, sum x, |r|_inf                                            x p' r' rhat | x r
+// KC reads r' of the ring blocks too, mostly from L2.  Every element-wise value is computed by the same expression from the
+// same operands as in the five-kernel path above; only the partition of the dot products differs.  KA reads p and nu of
+// ring blocks, so it must not write them in place: (p, nu) alternate between (kp, knu) and (kz, kzr) by the parity of the
+// iteration count, which one captured iteration body of the graph WHILE node serves for every pass (iteration 0 reads
+// neither: p = r).  r stays in kr and r' in kt: KB reads r of ring blocks and writes r' to kt, KC reads r' of ring blocks
+// and writes r to kr, so neither writes a vector that another of its CTAs reads.
 #ifndef KTILE_CTAS
 #define KTILE_CTAS 2 // resident CTAs/SM k_p_spmv and k_x_final are register-bounded for (128 registers; at 3 (80) both spill)
 #endif
@@ -514,12 +514,14 @@ struct __align__(16) TileSmem {
 
 // Warp w holds the blocks tiles[4w .. 4w+3] in row layout (lane = block lane>>3, row lane&7): warps 0-3 the interior block
 // rows, warps 4-7 the W, E, S, N ring blocks.  v: the vector to precondition; on return the interior warps hold
-// out = A M v of their rows in chunk layout (zero for absent blocks).  All threads call.  Walls: ghost = own cell.
+// out = A M v of their rows in chunk layout (zero for absent blocks), and M v of the interior blocks stays in the plane
+// until the next call's first CTA barrier; warps 4-7 return right after the plane is complete (out unset).  All threads
+// call.  Walls: ghost = own cell.
 __device__ __forceinline__ void tile_precond_lap(double (&v)[8], TileSmem &ts, double *sw, int lane, int warp,
                                                  const int *__restrict__ tslots, double2 (&out)[4]) {
   precond_row(v, sw, lane);
   const int bx = lane >> 3, y = lane & 7;
-  __syncthreads(); // the previous tile's stencil reads of the plane are done
+  __syncthreads(); // the previous tile's reads of the plane are done
   if (warp < 4) {
     double2 *p = reinterpret_cast<double2 *>(ts.plane + (warp * 8 + y + 1) * PST + bx * 8);
 #pragma unroll
@@ -574,7 +576,7 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
          const int *__restrict__ tiles, int ntiles, KrylovState *st, double *partials, unsigned int *counter, Comm comm) {
   if (st->done) return;
   const double beta = st->beta, nomega = -st->omega;
-  const bool restart = st->restart_now != 0;
+  const bool restart = st->restart_now != 0, first = st->iter == 0;
   const int in = pair_in(st);
   const double *__restrict__ p = in ? p1 : p0;
   const double *__restrict__ nu = in ? nu1 : nu0;
@@ -595,10 +597,10 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
     if (warp < 4 && !restart) blocks_stage(stg, rhat, sl, lane);
     double2 cp[4], cr[4], ch[4];
     blocks_ld(r, sl, lane, cr);
-    if (restart) {
+    if (restart || first) { // p = r, as in k_pupdate
 #pragma unroll
       for (int j = 0; j < 4; j++) cp[j] = ch[j] = cr[j];
-      if (warp < 4) blocks_st(rhat, sl, lane, cr);
+      if (restart && warp < 4) blocks_st(rhat, sl, lane, cr);
     } else {
       double2 cn[4];
       blocks_ld(p, sl, lane, cp);
@@ -642,8 +644,9 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
 #define KR_CTAS 3
 #endif
 // ---- KB: r' = r - alpha nu' ; t = A M r' ; t.r', t.t -> omega   (cuda.cu:499-518) -------------------------------------
+// Stores r' (not t): k_x_final recomputes t on its tile, which costs less than writing t and reading it back.
 __global__ void __launch_bounds__(NT, KR_CTAS)
-k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, double *__restrict__ t,
+k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, double *__restrict__ rp,
          const int *__restrict__ tiles, int ntiles, KrylovState *st, double *partials, unsigned int *counter, Comm comm) {
   if (st->done) return;
   const double alpha = st->alpha;
@@ -662,6 +665,7 @@ k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, dou
       cr[j].x = fma(-alpha, cn[j].x, cr[j].x);
       cr[j].y = fma(-alpha, cn[j].y, cr[j].y);
     }
+    if (warp < 4) blocks_st(rp, sl, lane, cr);
     double v[8];
     chunk_to_rows(sw, lane, cr, v);
     double2 ca[4];
@@ -674,7 +678,6 @@ k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, dou
         sums[1] = fma(ca[j].x, ca[j].x, sums[1]);
         sums[1] = fma(ca[j].y, ca[j].y, sums[1]);
       }
-      blocks_st(t, sl, lane, ca);
     }
   }
   grid_reduce<2, NT>(sums, 0.0, partials, counter, comm, [=](const double *tsum, double) {
@@ -684,60 +687,81 @@ k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, dou
   });
 }
 
-// ---- KC: r' = r - alpha nu' ; x = (x + alpha M p') + omega M r' ; r = r' - omega t ; rhat.r, |r|^2, sum x, |r|_inf ----------
-// Block-local, so it keeps the chunk loop of k_final.  It writes r in place: every ring reader of r (k_r_spmv) has finished.
+// ---- KC: t = A M r' ; x = (x + alpha M p') + omega M r' ; r = r' - omega t ; rhat.r, |r|^2, sum x, |r|_inf --------------
+// t is recomputed on the tile from the r' that k_r_spmv stored.  Warps 0-3 then hold t of the interior block rows and form
+// r; warps 4-7, done with their ring blocks, form x of interior block row warp-4 from z_p = M p' and from z_r, which they
+// read from the plane (rows 1..32, chunk layout).  The plane is overwritten only after the next tile's first CTA barrier,
+// which every warp reaches after it has finished this tile.  When the tile starts, warps 0-3 copy r^ into a stage (as
+// k_p_spmv does) and keep r' in registers, and warps 4-7 keep p'; x is loaded after the stencil: held across the tile
+// with the others it would cost spills.
 __global__ void __launch_bounds__(NT, KTILE_CTAS)
-k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1, const double *nu0, const double *nu1,
-          double *__restrict__ r, const double *__restrict__ t, const double *__restrict__ rhat, int nrows,
+k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1, double *__restrict__ r,
+          const double *__restrict__ rp, const double *__restrict__ rhat, const int *__restrict__ tiles, int ntiles,
           KrylovState *st, double *partials, unsigned int *counter, Comm comm, unsigned long long loop_handle) {
-  __shared__ __align__(16) double s_scr[WPB * SCR1];
   if (st->done) return;
   const double alpha = st->alpha, omega = st->omega;
   const int cur = st->cur, nxt = next_buf(st->cur, st->opt);
   const double *xc = cur == 0 ? x0 : (cur == 1 ? x1 : x2);
   double *xn = nxt == 0 ? x0 : (nxt == 1 ? x1 : x2);
-  const bool in = pair_in(st);
-  const double *__restrict__ p = in ? p0 : p1;
-  const double *__restrict__ nu = in ? nu0 : nu1;
+  const double *__restrict__ p = pair_in(st) ? p0 : p1; // what k_p_spmv of this iteration wrote
   double sums[3] = {0, 0, 0}; // rhat.r, r.r, sum x
   double mx = 0;
-  CHUNK_LOOP() {
-    const int nv = min(32, nrows - row0);
-    double2 cz[4], cy[4], cr[4], cn[4];
+  __shared__ __align__(16) double2 s_rhat[2 * 4 * 128]; // two stages, alternating by tile (see k_p_spmv)
+  int par = 0;
+  TILE_LOOP() {
+    const int *ts = tiles + (size_t)tile * TILE_SLOTS;
+    int sl[4], il[4]; // the warp's blocks; the interior blocks of block row warp & 3
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      sl[j] = ts[4 * warp + j];
+      il[j] = ts[4 * (warp & 3) + j];
+    }
+    double2 *stg = s_rhat + (par * 4 + (warp & 3)) * 128;
+    if (warp < 4) blocks_stage(stg, rhat, sl, lane);
+    double2 cr[4], ca[4]; // ca: r' (warps 0-3) or p' (warps 4-7) of block row warp & 3
+    blocks_ld(rp, sl, lane, cr);
+    if (warp < 4) {
+#pragma unroll
+      for (int j = 0; j < 4; j++) ca[j] = cr[j];
+    } else {
+      blocks_ld(p, il, lane, ca);
+    }
     double v[8];
-    chunk_ld(p, row0, nv, lane, cz);
-    chunk_ld(r, row0, nv, lane, cr);
-    chunk_ld(nu, row0, nv, lane, cn);
-    chunk_to_rows(sw, lane, cz, v);
-    precond_row(v, sw, lane);
-    rows_to_chunk(sw, lane, v, cz); // z_p
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      cr[j].x = fma(-alpha, cn[j].x, cr[j].x);
-      cr[j].y = fma(-alpha, cn[j].y, cr[j].y);
-    }
     chunk_to_rows(sw, lane, cr, v);
-    precond_row(v, sw, lane);
-    rows_to_chunk(sw, lane, v, cy); // z_r
-    double2 cx[4], ct[4], ch[4];
-    chunk_ld(xc, row0, nv, lane, cx);
-    chunk_ld(t, row0, nv, lane, ct);
-    chunk_ld(rhat, row0, nv, lane, ch);
+    double2 ct[4];
+    tile_precond_lap(v, s_tile, sw, lane, warp, ts, ct);
+    if (warp < 4) {
+      double2 ch[4];
+      stage_wait();
+      blocks_unstage(stg, sl, lane, ch);
 #pragma unroll
-    for (int j = 0; j < 4; j++) {
-      cx[j].x = fma(omega, cy[j].x, fma(alpha, cz[j].x, cx[j].x)); // cuda.cu:498 then 520
-      cx[j].y = fma(omega, cy[j].y, fma(alpha, cz[j].y, cx[j].y));
-      cr[j].x = fma(-omega, ct[j].x, cr[j].x); // cuda.cu:524
-      cr[j].y = fma(-omega, ct[j].y, cr[j].y);
-      sums[0] = fma(ch[j].x, cr[j].x, sums[0]);
-      sums[0] = fma(ch[j].y, cr[j].y, sums[0]);
-      sums[1] = fma(cr[j].x, cr[j].x, sums[1]);
-      sums[1] = fma(cr[j].y, cr[j].y, sums[1]);
-      sums[2] += cx[j].x + cx[j].y;
-      mx = fmax(mx, fmax(fabs(cr[j].x), fabs(cr[j].y)));
+      for (int j = 0; j < 4; j++) {
+        ca[j].x = fma(-omega, ct[j].x, ca[j].x); // cuda.cu:524
+        ca[j].y = fma(-omega, ct[j].y, ca[j].y);
+        sums[0] = fma(ch[j].x, ca[j].x, sums[0]);
+        sums[0] = fma(ch[j].y, ca[j].y, sums[0]);
+        sums[1] = fma(ca[j].x, ca[j].x, sums[1]);
+        sums[1] = fma(ca[j].y, ca[j].y, sums[1]);
+        mx = fmax(mx, fmax(fabs(ca[j].x), fabs(ca[j].y)));
+      }
+      blocks_st(r, sl, lane, ca);
+    } else {
+      double2 cx[4];
+      blocks_ld(xc, il, lane, cx);
+      chunk_to_rows(sw, lane, ca, v);
+      precond_row(v, sw, lane);
+      rows_to_chunk(sw, lane, v, ca); // z_p
+      const double2 *zr = reinterpret_cast<const double2 *>(s_tile.plane + ((warp - 4) * 8 + (lane >> 2) + 1) * PST) + (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const double2 z = zr[4 * j]; // z_r of block j, piece `lane`
+        cx[j].x = fma(omega, z.x, fma(alpha, ca[j].x, cx[j].x)); // cuda.cu:498 then 520
+        cx[j].y = fma(omega, z.y, fma(alpha, ca[j].y, cx[j].y));
+        sums[2] += cx[j].x + cx[j].y;
+      }
+      blocks_st(xn, il, lane, cx);
     }
-    chunk_st(xn, row0, nv, lane, cx);
-    chunk_st(r, row0, nv, lane, cr);
+    par ^= 1;
   }
   grid_reduce<3, NT>(sums, mx, partials, counter, comm, [=](const double *tsum, double m) {
     end_of_iteration(st, tsum, m, nxt);
@@ -775,12 +799,12 @@ int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts
   {
     ProfScope prof(s, KC_KINIT);
     if (has_irr)
-      k_init<true><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_TMP], s->f[CUP2D_PRES], s->kx[0], s->kr, s->krhat, s->kp,
-                                               s->knu, nbr, nrows, s->d_state, s->d_partials, s->d_counter,
+      k_init<true><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_TMP], s->f[CUP2D_PRES], s->kx[0], s->kr, s->krhat, nbr,
+                                               nrows, s->d_state, s->d_partials, s->d_counter,
                                                s->comm, irr_view(s), s->cond_handle);
     else
-      k_init<false><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_TMP], s->f[CUP2D_PRES], s->kx[0], s->kr, s->krhat, s->kp,
-                                                s->knu, nbr, nrows, s->d_state, s->d_partials, s->d_counter,
+      k_init<false><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_TMP], s->f[CUP2D_PRES], s->kx[0], s->kr, s->krhat, nbr,
+                                                nrows, s->d_state, s->d_partials, s->d_counter,
                                                 s->comm, irr_view(s), s->cond_handle);
   }
   s->launches += 2;
@@ -813,8 +837,8 @@ int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream) {
       }
       {
         ProfScope prof(s, KC_X_FINAL);
-        k_x_final<<<grid, NT, 0, stream>>>(s->kx[0], s->kx[1], s->kx[2], s->kp, s->kz, s->knu, s->kzr, s->kr, s->kt, s->krhat,
-                                           nrows, s->d_state, s->d_partials, s->d_counter, s->comm, s->cond_handle);
+        k_x_final<<<tgrid, NT, 0, stream>>>(s->kx[0], s->kx[1], s->kx[2], s->kp, s->kz, s->kr, s->kt, s->krhat, s->d_tiles,
+                                            s->ntiles, s->d_state, s->d_partials, s->d_counter, s->comm, s->cond_handle);
       }
       s->launches += 3;
     }
