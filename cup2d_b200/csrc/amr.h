@@ -27,6 +27,12 @@ int cup2d_amr_laplacian_fast(cup2d_amr *a, double dt);
 
 namespace cup2d {
 
+// One shape's obstacle blocks on the device (cup2d_shape_set, cup2d_amr_shape_set; csrc/penalize.cu): the ids of the nob
+// blocks its body touches, per block its chi X[8][8] and u_def[8][8][2]; room for cap blocks.  Kept here, not in sim.h, so
+// that cup2d_amr::Shape below can extend it where only this header is seen.
+struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr; };
+inline void shape_free(Shape &sh) { cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); }
+
 constexpr int AMR_GRID_SMS = 132; // SMs of an H100 SXM: the grid-stride launches of this path are capped at a few waves of them
 
 struct Csr {
@@ -86,7 +92,7 @@ struct cup2d_amr;
 extern "C" int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max);
 // single-rank contexts: the fast path's neighbour / irregular-block / compact ghost tables (csrc/amr_fast.cu), built on first use
 int amr_fast_tables(cup2d_amr *a);
-// the per-block (i, j) table on the device, built on first use (csrc/amr_penalize.cu)
+// the per-block (i, j) table on the device, built on first use (csrc/penalize.cu)
 int amr_ensure_ij(cup2d_amr *a);
 // distributed contexts (cup2d_amr_create_ranks): refresh the halo slots of `field` from the owners (whole-block peer pulls,
 // csrc/halo.cu) before a kernel reads neighbours; a no-op otherwise
@@ -135,11 +141,11 @@ struct cup2d_amr {
                                     // 3 and 6 (the force diagnostics' labs, csrc/amr_forces.cu) on first use
   int *d_nbr8 = nullptr;            // [nb][8] cup2d_amr_plan_neighbours on the device (csrc/amr_forces.cu, first use)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)
-  // bodies (csrc/amr_penalize.cu): per-shape obstacle blocks, as cup2d_sim::Shape
+  // bodies (csrc/penalize.cu): per-shape obstacle blocks, a cup2d::Shape with
   // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid or given one by cup2d_amr_shape_set_dist;
   // ascending: the block ids are strictly ascending, recorded by cup2d_amr_shape_set, always true after cup2d_amr_ongrid)
   // (has_surface: cup2d_amr_surface has run on the shape as it stands; cup2d_amr_shape_set and cup2d_amr_ongrid clear it)
-  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr, *d_dist = nullptr; bool has_dist = false, ascending = true, has_surface = false; };
+  struct Shape : cup2d::Shape { double *d_dist = nullptr; bool has_dist = false, ascending = true, has_surface = false; };
   std::vector<Shape> shapes;
   std::vector<int32_t> h_ij;        // [nb][2] block index (i, j) at the block's own level (filled by cup2d_amr_create)
   int *d_ij = nullptr;              // the same on the device (first use)
@@ -178,7 +184,8 @@ struct cup2d_amr {
   bool step_pending = false;        // an enqueued step / pressure section whose result has not been read
   void free_shapes() {
     for (auto &sh : shapes) {
-      cudaFree(sh.d_ids); cudaFree(sh.d_X); cudaFree(sh.d_udef); cudaFree(sh.d_dist);
+      cup2d::shape_free(sh);
+      cudaFree(sh.d_dist);
     }
     shapes.clear();
     cudaFree(d_ij); cudaFree(d_shape_part);

@@ -12,14 +12,6 @@ static thread_local std::string g_err;
 void set_error(const std::string &msg) { g_err = msg; }
 int dim_of(int field) { return (field == CUP2D_VEL || field == CUP2D_VOLD || field == CUP2D_TMPV) ? 2 : 1; }
 
-#define CUP2D_REQUIRE(cond, msg)                                                                  \
-  do {                                                                                            \
-    if (!(cond)) {                                                                                \
-      cup2d::set_error(msg);                                                                      \
-      return CUP2D_EINVAL;                                                                        \
-    }                                                                                             \
-  } while (0)
-
 // ---- space-filling curve: host restatement of SpaceCurve (main.cpp:342-446, init 6342-6376) ------
 static long long hilbert_xy2d(int b, int x, int y) { // AxestoTranspose, main.cpp:347-359
   const int n = 1 << b;

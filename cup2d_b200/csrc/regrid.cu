@@ -7,8 +7,11 @@
 //  * cup2d_dump: the reference's dump() (main.cpp:3367-3467), same three files byte for byte: the float32 quad
 //      corners and (u, v, 0) attributes are produced on the device in `infos` order and streamed through a pinned
 //      staging buffer into the files (every rank writes its own byte range, as MPI_File_write_at_all does).
+//      cup2d_amr_dump writes the same files from a multi-level mesh.
 #include "rows.cuh"
 #include "sim.h"
+#include "amr.h"
+#include <algorithm>
 #include <cstdio>
 #include <fcntl.h>
 #include <string>
@@ -181,18 +184,20 @@ int launch_adapt_tags(cup2d_sim *s, double rtol, int chi_cells, double *linf_hos
 // ------------------------------------------------------------------------------------------------
 // dump(): one thread per cell of blocks [b0, b0+nb): 8 floats of quad corners + 3 floats of attribute
 // (main.cpp:3431-3452).  origin = i*8*h0/2^level (main.cpp:695-696) = (8 i) h exactly (power-of-two scaling);
-// no FMA contraction anywhere so that the doubles, and hence the narrowed floats, are the reference's.
+// no FMA contraction anywhere so that the doubles, and hence the narrowed floats, are the reference's.  The cell size
+// of block id is hb[id] on a multi-level mesh (hb != nullptr), h on the uniform grid.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-dump_pack_kernel(const double *__restrict__ vel, const int2 *__restrict__ ij, double h, int b0, int nb,
-                 float4 *__restrict__ xyz, float *__restrict__ attr) {
+dump_pack_kernel(const double *__restrict__ vel, const int2 *__restrict__ ij, const double *__restrict__ hb, double h,
+                 int b0, int nb, float4 *__restrict__ xyz, float *__restrict__ attr) {
   const size_t ncell = (size_t)nb * 64;
   for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < ncell; i += (size_t)gridDim.x * 256) {
     const int k = (int)(i >> 6), x = (int)(i & 7), y = (int)((i >> 3) & 7);
     const int2 b = ij[b0 + k];
-    const double u0 = __dadd_rn(__dmul_rn((double)(b.x * CUP2D_BS), h), __dmul_rn(h, (double)x));
-    const double v0 = __dadd_rn(__dmul_rn((double)(b.y * CUP2D_BS), h), __dmul_rn(h, (double)y));
-    const float fu0 = (float)u0, fv0 = (float)v0, fu1 = (float)__dadd_rn(u0, h), fv1 = (float)__dadd_rn(v0, h);
+    const double hk = hb ? hb[b0 + k] : h;
+    const double u0 = __dadd_rn(__dmul_rn((double)(b.x * CUP2D_BS), hk), __dmul_rn(hk, (double)x));
+    const double v0 = __dadd_rn(__dmul_rn((double)(b.y * CUP2D_BS), hk), __dmul_rn(hk, (double)y));
+    const float fu0 = (float)u0, fv0 = (float)v0, fu1 = (float)__dadd_rn(u0, hk), fv1 = (float)__dadd_rn(v0, hk);
     xyz[2 * i] = make_float4(fu0, fv0, fu0, fv1);
     xyz[2 * i + 1] = make_float4(fu1, fv1, fu1, fv0);
     const double2 q = reinterpret_cast<const double2 *>(vel)[(size_t)(b0 + k) * 64 + (i & 63)];
@@ -202,7 +207,7 @@ dump_pack_kernel(const double *__restrict__ vel, const int2 *__restrict__ ij, do
   }
 }
 
-int dump_write_all(int fd, const void *buf, size_t n, off_t off) {
+static int dump_write_all(int fd, const void *buf, size_t n, off_t off) {
   const char *p = static_cast<const char *>(buf);
   while (n > 0) {
     const ssize_t w = pwrite(fd, p, n, off);
@@ -215,8 +220,8 @@ int dump_write_all(int fd, const void *buf, size_t n, off_t off) {
 }
 
 // the .xdmf2 descriptor of dump() (main.cpp:3380-3423), byte for byte
-int dump_write_xdmf(const std::string &xdmf_path, const std::string &xyz_path, const std::string &attr_path, double time,
-                    long ncell_total) {
+static int dump_write_xdmf(const std::string &xdmf_path, const std::string &xyz_path, const std::string &attr_path, double time,
+                           long ncell_total) {
   auto basename_of = [](const std::string &p) { // main.cpp:3380-3385: after the last '/' that is not the final char
     size_t cut = 0;
     for (size_t j = 0; j + 1 < p.size(); j++)
@@ -241,52 +246,77 @@ int dump_write_xdmf(const std::string &xdmf_path, const std::string &xyz_path, c
   return CUP2D_OK;
 }
 
-int dump_fields(cup2d_sim *s, double time, const char *path) {
+// dump()'s three files path.xdmf2 / .xyz.raw / .attr.raw of the velocity `vel` of nb blocks, which are blocks
+// [gbegin, gbegin + nb) of the nglobal blocks of the whole mesh: every rank writes its own byte range, as
+// MPI_File_write_at_all does, and one of them (write_xdmf) the descriptor (main.cpp:3387-3390).  ij: (i, j) per block;
+// hb / h: the cell size as in dump_pack_kernel; oflags: open() flags of the two raw files; grid_cap: the pack kernel's
+// grid cap; who: the prefix of the error messages; launches (may be null): counts the pack kernel launches.
+static int dump_write(cudaStream_t stream, const double *vel, const int *ij, const double *hb, double h, int64_t nb,
+                      int64_t gbegin, int64_t nglobal, bool write_xdmf, int oflags, int grid_cap, const char *who,
+                      double time, const char *path, int64_t *launches) {
   const std::string base(path);
   const std::string xyz_path = base + ".xyz.raw", attr_path = base + ".attr.raw", xdmf_path = base + ".xdmf2";
-  if (s->rank == s->nranks - 1) { // main.cpp:3390: the last rank writes the descriptor
-    const int rc = dump_write_xdmf(xdmf_path, xyz_path, attr_path, time, (long)s->nglobal * 64);
-    if (rc) return rc;
-  }
-  {
-    const int rc = ensure_block_ij(s);
+  if (write_xdmf) {
+    const int rc = dump_write_xdmf(xdmf_path, xyz_path, attr_path, time, (long)nglobal * 64);
     if (rc) return rc;
   }
   // staging: CHUNK blocks at a time, device + pinned host (44 B per cell)
-  const int CHUNK = (int)std::min<int64_t>(s->nloc, 16384);
-  const size_t cx = (size_t)CHUNK * 64 * 8 * sizeof(float), ca = (size_t)CHUNK * 64 * 3 * sizeof(float);
+  const int CHUNK = (int)std::min<int64_t>(nb, 16384);
+  const size_t nx = (size_t)CHUNK * 64 * 8, na = (size_t)CHUNK * 64 * 3;
   float *d_buf = nullptr, *h_buf = nullptr;
-  CUP2D_CUDA(cudaMalloc(&d_buf, cx + ca));
-  if (cudaMallocHost(&h_buf, cx + ca) != cudaSuccess) {
+  CUP2D_CUDA(cudaMalloc(&d_buf, (nx + na) * sizeof(float)));
+  if (cudaMallocHost(&h_buf, (nx + na) * sizeof(float)) != cudaSuccess) {
     cudaFree(d_buf);
-    set_error("dump: cannot allocate the pinned staging buffer");
+    set_error(std::string(who) + ": cannot allocate the pinned staging buffer");
     return CUP2D_ECUDA;
   }
-  const int fx = open(xyz_path.c_str(), O_CREAT | O_WRONLY, 0644), fa = open(attr_path.c_str(), O_CREAT | O_WRONLY, 0644);
-  int rc = CUP2D_OK;
-  if (fx < 0 || fa < 0) rc = CUP2D_EINVAL;
-  for (int64_t b0 = 0; rc == CUP2D_OK && b0 < s->nloc; b0 += CHUNK) {
-    const int nb = (int)std::min<int64_t>(CHUNK, s->nloc - b0);
-    const size_t ncell = (size_t)nb * 64;
-    float *dx = d_buf, *da = d_buf + (size_t)CHUNK * 64 * 8;
-    dump_pack_kernel<<<std::min<int>((int)((ncell + 255) / 256), s->num_sms * 8), 256, 0, s->stream>>>(
-        s->f[CUP2D_VEL], reinterpret_cast<const int2 *>(s->d_ij), s->h, (int)b0, nb, reinterpret_cast<float4 *>(dx), da);
-    s->launches++;
-    cudaMemcpyAsync(h_buf, dx, ncell * 8 * sizeof(float), cudaMemcpyDeviceToHost, s->stream);
-    cudaMemcpyAsync(h_buf + (size_t)CHUNK * 64 * 8, da, ncell * 3 * sizeof(float), cudaMemcpyDeviceToHost, s->stream);
-    if (cudaStreamSynchronize(s->stream) != cudaSuccess) { rc = CUP2D_ECUDA; break; }
-    const off_t cell0 = (off_t)(s->gbegin + b0) * 64; // MPI_Exscan offset (main.cpp:3387) + position in the range
+  const int fx = open(xyz_path.c_str(), oflags, 0644), fa = open(attr_path.c_str(), oflags, 0644);
+  int rc = (fx < 0 || fa < 0) ? CUP2D_EINVAL : CUP2D_OK;
+  for (int64_t b0 = 0; rc == CUP2D_OK && b0 < nb; b0 += CHUNK) {
+    const int n = (int)std::min<int64_t>(CHUNK, nb - b0);
+    const size_t ncell = (size_t)n * 64;
+    dump_pack_kernel<<<(int)std::min<size_t>((ncell + 255) / 256, grid_cap), 256, 0, stream>>>(
+        vel, reinterpret_cast<const int2 *>(ij), hb, h, (int)b0, n, reinterpret_cast<float4 *>(d_buf), d_buf + nx);
+    if (launches) ++*launches;
+    cudaMemcpyAsync(h_buf, d_buf, ncell * 8 * sizeof(float), cudaMemcpyDeviceToHost, stream);
+    cudaMemcpyAsync(h_buf + nx, d_buf + nx, ncell * 3 * sizeof(float), cudaMemcpyDeviceToHost, stream);
+    if (cudaStreamSynchronize(stream) != cudaSuccess) {
+      rc = CUP2D_ECUDA;
+      break;
+    }
+    const off_t cell0 = (off_t)(gbegin + b0) * 64; // MPI_Exscan offset (main.cpp:3387) + position in the range
     if (dump_write_all(fx, h_buf, ncell * 8 * sizeof(float), cell0 * 8 * (off_t)sizeof(float)) ||
-        dump_write_all(fa, h_buf + (size_t)CHUNK * 64 * 8, ncell * 3 * sizeof(float), cell0 * 3 * (off_t)sizeof(float)))
+        dump_write_all(fa, h_buf + nx, ncell * 3 * sizeof(float), cell0 * 3 * (off_t)sizeof(float)))
       rc = CUP2D_EINVAL;
   }
   if (fx >= 0) close(fx);
   if (fa >= 0) close(fa);
   cudaFreeHost(h_buf);
   cudaFree(d_buf);
-  if (rc == CUP2D_EINVAL) set_error("dump: cannot write " + xyz_path + " / " + attr_path);
-  if (rc == CUP2D_ECUDA) set_error(std::string("dump: ") + cudaGetErrorString(cudaGetLastError()));
+  if (rc == CUP2D_EINVAL) set_error(std::string(who) + ": cannot write " + xyz_path + " / " + attr_path);
+  if (rc == CUP2D_ECUDA) set_error(std::string(who) + ": " + cudaGetErrorString(cudaGetLastError()));
   return rc;
 }
 
+int dump_fields(cup2d_sim *s, double time, const char *path) {
+  const int rc = ensure_block_ij(s);
+  if (rc) return rc;
+  // main.cpp:3390: the last rank writes the descriptor; the files are not truncated
+  return dump_write(s->stream, s->f[CUP2D_VEL], s->d_ij, nullptr, s->h, s->nloc, s->gbegin, s->nglobal,
+                    s->rank == s->nranks - 1, O_CREAT | O_WRONLY, s->num_sms * 8, "dump", time, path, &s->launches);
+}
+
 } // namespace cup2d
+
+/* dump() of the velocity on a multi-level mesh (main.cpp:3367-3467): the three files of cup2d_dump, byte for byte, with
+ * the cell size of every block its own */
+extern "C" int cup2d_amr_dump(cup2d_amr *a, double time, const char *path) {
+  CUP2D_REQUIRE(a != nullptr && path && *path, "cup2d_amr_dump: bad arguments");
+  CUP2D_CUDA(cudaSetDevice(a->device));
+  const int rc = amr_ensure_ij(a);
+  if (rc) return rc;
+  const bool dist = a->dist && a->nranks > 1; // every rank writes its own byte range, the last one the descriptor
+  return cup2d::dump_write(a->stream, a->f[CUP2D_VEL], a->d_ij, a->d_h, 0, a->nb, dist ? a->gbegin : 0,
+                           dist ? a->nglobal : a->nb, !dist || a->rank == a->nranks - 1, O_CREAT | O_WRONLY | (dist ? 0 : O_TRUNC),
+                           cup2d::AMR_GRID_SMS * 8, "cup2d_amr_dump", time, path, nullptr);
+}

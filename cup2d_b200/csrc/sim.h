@@ -3,14 +3,22 @@
 #include "../../include/cup2d_b200.h"
 #include "common.cuh"
 #include "rows.cuh"
+#include "amr.h" // the multi-level context, and the shape record both contexts keep
 #include <mutex>
 #include <string>
-#include <sys/types.h>
 #include <vector>
+
+#define CUP2D_REQUIRE(cond, msg)                                                                  \
+  do {                                                                                            \
+    if (!(cond)) {                                                                                \
+      cup2d::set_error(msg);                                                                      \
+      return CUP2D_EINVAL;                                                                        \
+    }                                                                                             \
+  } while (0)
 
 namespace cup2d {
 
-constexpr int TILE_B = 4;                 // advect tile = 4x4 blocks = 32x32 cells
+constexpr int TILE_B = 4;                // advect tile = 4x4 blocks = 32x32 cells
 constexpr int TILE_SLOTS = 32;            // 16 interior + 4 W + 4 E + 4 S + 4 N
 constexpr int MAX_RANKS = 8;
 constexpr int RED_MAX_CTAS = 4096;        // upper bound on reduction grid size
@@ -122,8 +130,7 @@ struct cup2d_sim {
   double *d_irr_val = nullptr;
   int64_t n_irr_rows = 0;
   // bodies: per-shape obstacle blocks on the device (cup2d_shape_set)
-  struct Shape { int nob = 0, cap = 0; int *d_ids = nullptr; double *d_X = nullptr, *d_udef = nullptr; };
-  std::vector<Shape> shapes;
+  std::vector<cup2d::Shape> shapes;
   // host-buffer pipeline (cup2d_pipe_*): staging sets, copy streams, ordering events
   struct PipeSet { double *vel = nullptr, *pres = nullptr; cudaEvent_t in_done = nullptr, step_done = nullptr, out_done = nullptr; };
   PipeSet pipe[CUP2D_PIPE_SLOTS];
@@ -211,7 +218,4 @@ int poisson_create_general_ranks_ex(int64_t nblocks_global, int32_t rank, int32_
                                     const int32_t *nbr, int64_t n_irr, const int32_t *irr_rows, const int32_t *irr_rowptr,
                                     const int32_t *irr_col, const double *irr_val, int64_t n_extra,
                                     const int32_t *extra_blocks, int32_t device, cup2d_sim **out);
-int dump_write_xdmf(const std::string &xdmf_path, const std::string &xyz_path, const std::string &attr_path, double time,
-                    long ncell_total);
-int dump_write_all(int fd, const void *buf, size_t n, off_t off);
 } // namespace cup2d

@@ -42,15 +42,16 @@ def test_gpu_parity_subset_on_the_emulated_library(emulated_library):
     assert n >= 12, tail
 
 
-def test_two_ranks_emulated_in_one_process(emulated_library):
+def test_two_ranks_emulated_in_one_process(emulated_library, tmp_path):
     """the multi-GPU path (peer-memory halo pulls with ready flags, in-kernel all-reduce of the Krylov dots, SFC-range
     partition) with the two ranks running as threads of one process: their 'device' buffers are mapped into each other through
-    the emulated IPC handles and their kernels really run concurrently.  2 steps x 10 Poisson iterations vs the oracle."""
+    the emulated IPC handles and their kernels really run concurrently.  2 steps x 10 Poisson iterations vs the oracle, then
+    dump() from both ranks into one set of files (each rank its own byte range, the last one the descriptor) vs the oracle's."""
     code = r'''
 import sys, threading, numpy as np
 sys.path.insert(0, %r); sys.path.insert(0, %r)
 import cup2d_b200, cup2d_oracle as orc
-W, L = 2, 3
+W, L, pref = 2, 3, %r
 N = 8 << L
 x = (np.arange(N) + 0.5) / N
 X, Y = np.meshgrid(x, x)
@@ -75,6 +76,7 @@ def run(rank):
             dt, it, err = sim.step(max_iter=10)
             outs.append((dt, sim.download_blocks("vel"), sim.download_blocks("pres")))
             bar.wait()
+        sim.dump(0.25, pref)
         res[rank] = (sim.order, sim.nbx, sim.nby, outs)
         bar.wait(); sim.close()
     except Exception as e:
@@ -91,9 +93,12 @@ for s in range(2):
     worst = max(worst, abs(res[0][3][s][0] - ref["dt"]) / ref["dt"], np.abs(gu - ref["u"]).max(), np.abs(gv - ref["v"]).max(),
                 np.abs(gp - ref["p"]).max())
     ru, rv, rp = ref["u"], ref["v"], ref["p"]
+xyz, attr = orc.dump_arrays(gu, gv, order, 1.0 / 8, L)
+assert open(pref + ".xyz.raw", "rb").read() == xyz.tobytes() and open(pref + ".attr.raw", "rb").read() == attr.tobytes()
+assert open(pref + ".xdmf2").read() == orc.dump_xdmf(0.25, len(order) * 64, "dump.xyz.raw", "dump.attr.raw")
 print("WORST", worst)
 assert worst < 1e-12
-''' % (ROOT, os.path.join(ROOT, "oracle"))
+''' % (ROOT, os.path.join(ROOT, "oracle"), str(tmp_path / "dump"))
     r = subprocess.run([sys.executable, "-c", code], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900,
                        env=dict(os.environ, CUP2D_B200_LIB=emulated_library))
     assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
@@ -277,20 +282,21 @@ assert worst < 1e-11
     assert r.returncode == 0 and "WORST" in r.stdout, r.stdout[-1500:]
 
 
-def test_distributed_multi_level_mesh_on_three_ranks_emulated(emulated_library):
+def test_distributed_multi_level_mesh_on_three_ranks_emulated(emulated_library, tmp_path):
     """several GPUs on a multi-level mesh, second form (cup2d_amr_create_ranks): the mesh itself is distributed by block ranges;
     every rank holds its blocks plus halo slots for the remote blocks its tables name (face neighbours, ghost-row sources, fine
     sides of its coarse faces, Poisson columns), refreshed by whole-block peer pulls; face fluxes cross rank boundaries inside a
     field array; dt and the pressure means are all-reduced in a kernel.  Three ranks (uneven ranges) as threads of one process:
-    (1) on the reference's 7-level run.sh mesh the body sums / blend / u_def assembly against the one-rank context and the
-    flux-corrected operators and adapt()'s tagging field against the reference's own outputs; (2) two full steps on a
-    three-level mesh against the one-rank run."""
+    (1) on the reference's 7-level run.sh mesh the body sums / blend / u_def assembly / dump() files against the one-rank
+    context and the flux-corrected operators and adapt()'s tagging field against the reference's own outputs; (2) two full
+    steps on a three-level mesh against the one-rank run."""
     code = r'''
 import sys, threading, numpy as np
 sys.path.insert(0, %r); sys.path.insert(0, %r)
 import bench_amr
 from cup2d_b200.amr import AmrSimulation
 W = 3
+one_pref, rank_pref = %r, %r      # one file name in two directories: the descriptor names the files
 bar, slots, errs = threading.Barrier(W), [None] * W, []
 class Dist:
     def __init__(self, rank): self.rank = rank
@@ -319,6 +325,7 @@ one = AmrSimulation(blocks, int(d["bpdx"]), int(d["bpdy"]), float(d["h0"]), floa
 one.upload("vel", d["vel"]); one.upload("chi", d["chi"]); one.shape_set(0, ids, X, ud)
 want_q = one.shape_integrals(0, *body)
 one.penalize(0, *body, 0.1, -0.2, 0.7); want_v = one.download("vel"); one.udef_assemble(); want_t = one.download("tmpV")
+one.dump(0.25, one_pref)
 one.close()
 def ops(rank):
     sl, dt = slice(rb[rank], rb[rank + 1]), float(d["dt"])
@@ -328,6 +335,7 @@ def ops(rank):
     q = sim.shape_integrals(0, *body)                                   # all-reduced: the same seven sums on every rank
     sim.penalize(0, *body, 0.1, -0.2, 0.7); pv = sim.download("vel"); sim.udef_assemble(); pt = sim.download("tmpV")
     assert np.abs(q - want_q).max() <= 1e-12 * np.abs(want_q).max() and np.array_equal(pv, want_v[sl]) and np.array_equal(pt, want_t[sl])
+    sim.dump(0.25, rank_pref)                                           # every rank its own byte range, the last the descriptor
     sim.upload("vel", d["vel"][sl]); sim.advect_diffuse_rhs(dt); adv = sim.download("tmpV")
     sim.upload("tmpV", d["udef"][sl]); sim.upload("chi", d["chi"][sl]); sim.upload("pold", d["pres"][sl])
     sim.pressure_rhs(dt, True); rhs1 = sim.download("tmp")
@@ -335,6 +343,8 @@ def ops(rank):
     bar.wait(); sim.close()
     return adv, rhs1, gp
 res = on_ranks(ops)
+for ext in (".xyz.raw", ".attr.raw", ".xdmf2"):
+    assert open(rank_pref + ext, "rb").read() == open(one_pref + ext, "rb").read(), ext
 worst = 0.0
 for i, name in enumerate(("adv", "rhs1", "gradp")):
     got = np.concatenate([res[r][i] for r in range(W)])
@@ -381,8 +391,10 @@ for s in range(2):
     assert all(res[r][s][0] == res[0][s][0] for r in range(W)) and res[0][s][0][1] == ref[s][0][1] == 5
 print("WORST", worst)
 assert worst < 1e-11
-''' % (ROOT, os.path.join(ROOT, "tools"), os.path.join(ROOT, "tests", "golden", "amrlab_lmax8.npz"),
-       os.path.join(ROOT, "tests", "golden", "amrtags_lmax8.npz"))
+''' % (ROOT, os.path.join(ROOT, "tools"), str(tmp_path / "one" / "dump"), str(tmp_path / "ranks" / "dump"),
+       os.path.join(ROOT, "tests", "golden", "amrlab_lmax8.npz"), os.path.join(ROOT, "tests", "golden", "amrtags_lmax8.npz"))
+    (tmp_path / "one").mkdir()
+    (tmp_path / "ranks").mkdir()
     r = subprocess.run([sys.executable, "-c", code], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300,  # a rank that dies leaves the others spinning on its flags
                       
                        env=dict(os.environ, CUP2D_B200_LIB=emulated_library))

@@ -1,4 +1,4 @@
-"""GPU tests of the multi-level device path (csrc/amr_ops.cu baseline kernels, csrc/amr_fast.cu, csrc/amr_penalize.cu, the
+"""GPU tests of the multi-level device path (csrc/amr_ops.cu baseline kernels, csrc/amr_fast.cu, the bodies of csrc/penalize.cu, the
 tagging of cup2d_amr_adapt_tags) against the reference's own outputs on its 7-level run.sh mesh (tests/golden/amrlab_lmax8.npz,
 amrtags_lmax8.npz), against the reference restatement on a second mesh family, and in situ (the reference's run.sh case
 with its hot path spliced onto this path).
