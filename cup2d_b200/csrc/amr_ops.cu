@@ -1129,7 +1129,7 @@ static int enqueue_body(cup2d_amr *a, bool pressure_only, bool dev_dt, double cf
   CUP2D_CUDA(cudaStreamWaitEvent(ps->stream, (cudaEvent_t)a->ev_fork, 0));
   CUP2D_CUDA(cudaMemcpyAsync(ps->f[CUP2D_TMP], a->f[CUP2D_TMP], n * sizeof(double), cudaMemcpyDeviceToDevice, ps->stream));
   CUP2D_CUDA(cudaMemcpyAsync(ps->f[CUP2D_PRES], a->f[CUP2D_PRES], n * sizeof(double), cudaMemcpyDeviceToDevice, ps->stream));
-  if ((rc = poisson_enqueue(ps, tol_abs, tol_rel, max_restarts, max_iter, false, capturing))) return rc;
+  if ((rc = poisson_enqueue(ps, tol_abs, tol_rel, max_restarts, max_iter, capturing))) return rc;
   CUP2D_CUDA(cudaEventRecord((cudaEvent_t)a->ev_join, ps->stream));
   CUP2D_CUDA(cudaStreamWaitEvent(a->stream, (cudaEvent_t)a->ev_join, 0));
   amr_take_x_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], ps->kx[0], ps->kx[1], ps->kx[2], ps->d_state, n);

@@ -593,7 +593,7 @@ int64_t cup2d_launch_count(const cup2d_sim *s) { return s ? s->launches : 0; }
 
 static const char *kclass_name[KC_COUNT] = {"advect_stage_kernel", "umax_kernel", "pressure_rhs_kernel",
     "pressure_correct_kernel", "k_init", "k_pupdate", "k_spmv<0>", "k_r_update", "k_spmv<1>", "k_final",
-    "k_p_spmv", "k_r_spmv", "k_x_final", "halo_pull_kernel", "vorticity_tag_kernel"};
+    "k_p_spmv", "k_r_spmv", "k_x_final", "halo_pull_kernel", "vorticity_tag_kernel", "pressure_rhs_start_kernel"};
 int cup2d_profile_enable(cup2d_sim *s, int on) {
   if (!s) return CUP2D_EINVAL;
   s->prof.clear(); // the events stay in the pool and are reused
@@ -810,17 +810,18 @@ int cup2d_pressure_correct(cup2d_sim *s, double dt) {
 
 namespace cup2d {
 
-// The Krylov solve of an enqueued step on s->stream (b = tmp, x0 = pres; the iterate stays in the Krylov buffers, KrylovState::opt
-// names the best one).  Fixed work is queued at once; a tolerance-driven solve is, while `capturing`, a WHILE node whose
+// The Krylov solve of an enqueued step on s->stream (b = tmp and x0 = pres, or b formed from the step's right-hand side and
+// x0 = 0; the iterate stays in the Krylov buffers, KrylovState::opt names the best one).  Fixed work is queued at once; a tolerance-driven solve is, while `capturing`, a WHILE node whose
 // body is one iteration, and otherwise host-polled in batches of 8 (the only host waits, in direct launches only).
-int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current,
-                    bool capturing) {
+int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool capturing,
+                    const StepRhs *rhs) {
   const bool tol = tol_abs > 0 || tol_rel > 0;
 #ifndef CUP2D_FULL_EMU
   cudaGraph_t cap_graph = nullptr;
   if (capturing && tol && max_iter > 0) {
     // tolerance-driven solve inside a graph: a WHILE node whose body is one iteration.  Its condition starts at 1 on
-    // every launch; the last CTA of k_init and of every k_final / k_x_final sets it to !done (cudaGraphSetConditional).
+    // every launch; the last CTA of the starting kernel and of every k_final / k_x_final sets it to !done
+    // (cudaGraphSetConditional).
     cudaStreamCaptureStatus st;
     CUP2D_CUDA(cudaStreamGetCaptureInfo(s->stream, &st, nullptr, &cap_graph, nullptr, nullptr));
     cudaGraphConditionalHandle handle;
@@ -828,7 +829,8 @@ int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restar
     s->cond_handle = (unsigned long long)handle;
   }
 #endif
-  int rc = poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter, x0_halo_current);
+  int rc = rhs ? poisson_begin_rhs(s, tol_abs, tol_rel, max_restarts, max_iter, *rhs)
+               : poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter);
   if (rc) {
     s->cond_handle = 0;
     return rc;
@@ -902,8 +904,10 @@ static int step_body(cup2d_sim *s, bool dev_dt, int keep_udef, double tol_abs, d
   // keep_udef = 0: no bodies, the sum of u_def is identically zero (main.cpp:6980-6983), so the RHS
   // kernel skips the chi*div(u_def) term instead of reading a zeroed field (tmpV keeps RK scratch).
   // keep_udef = 1: the caller uploaded chi and the summed u_def into tmpV after the RK2 stages.
-  if ((rc = launch_pressure_rhs(s, 1.0, keep_udef != 0, s->d_fac, true))) return rc;
-  if ((rc = poisson_enqueue(s, tol_abs, tol_rel, max_restarts, max_iter, true, capturing))) return rc;
+  // The solve starts in the kernel that forms the right-hand side (x0 = 0): neither b nor x0 goes through tmp / pres, so
+  // after a step tmp does not hold b (cup2d_pressure_rhs still writes it there).
+  const StepRhs rhs{keep_udef != 0, s->d_fac};
+  if ((rc = poisson_enqueue(s, tol_abs, tol_rel, max_restarts, max_iter, capturing, &rhs))) return rc;
   return launch_pressure_correct(s, 1.0, s->d_fac, true);
 }
 

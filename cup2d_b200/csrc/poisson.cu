@@ -19,7 +19,7 @@
 // x' = x + alpha z of cuda.cu:498 is deferred into the final kernel, which applies x'' = (x + alpha z_p) + omega z_r
 // in the reference's order (bitwise the same iterate), so the middle kernel neither reads nor writes x or z_p.
 // Memory access: warp-cooperative coalesced rows through padded shared memory (rows.cuh).
-#include "rows.cuh"
+#include "rhs.cuh"
 #include "sim.h"
 #include <algorithm>
 #include <cmath>
@@ -229,6 +229,17 @@ __device__ __forceinline__ void set_loop_condition(unsigned long long handle, co
   double *sw = s_scr + warp * SCR1;                                                               \
   for (int row0 = (blockIdx.x * WPB + warp) * 32; row0 < nrows; row0 += gridDim.x * WPB * 32)
 
+// state of a solve after its start kernel, from the global |r|^2, sum(x0) and |r|_inf (cuda.cu:428-430)
+__device__ void start_of_solve(KrylovState *st, const double *t, double m, unsigned long long loop_handle) {
+  st->err = st->err_init = st->err_opt = m;
+  st->xsum = t[1];
+  st->nrh2 = t[0];
+  st->iter = 0;
+  if (st->max_iter <= 0) st->done = 1;
+  prepare_iteration(st, t[0], t[0]);
+  set_loop_condition(loop_handle, st);
+}
+
 // ---- K0: r = b - A x0 ; rhat = r ; x[0] = x0 ; err0, |r|^2, sum(x0) -----------------
 // p = nu = 0 is not stored: the first p-update of a solve (iter 0) takes p = r, which is beta*(0 - omega*0) + r.
 template <bool IRR>
@@ -258,14 +269,46 @@ k_init(const double *__restrict__ b, const double *__restrict__ x0, double *__re
     rows_store1(rhat, row0, nv, sw, lane, bb);
     rows_store1(x, row0, nv, sw, lane, xx);
   }
+  grid_reduce<2, NT>(sums, mx, partials, counter, comm,
+                     [=](const double *t, double m) { start_of_solve(st, t, m, loop_handle); });
+}
+
+// ---- K0 of a time step: b = fac*(div vel) - fac*chi*(div udef) - lap(pold) ; r = rhat = b ; x[0] = 0 ; err0, |r|^2 -------
+// k_init with x0 = 0 fused into the right-hand-side kernel: A*0 = +0 (for general rows too), so r = b - A*0 is b bit for
+// bit, and neither b nor x0 makes a round trip through tmp / pres.  Launched on k_init's grid with its row partition and
+// per-lane summation order, so |r|^2, |r|_inf and sum(x0) = +0 are bitwise what k_init returns for b and x0 = 0.
+template <bool HAS_UDEF>
+__global__ void __launch_bounds__(NT)
+pressure_rhs_start_kernel(const double *__restrict__ vel, const double *__restrict__ udef, const double *__restrict__ chi,
+                          const double *__restrict__ pold, double *__restrict__ x, double *__restrict__ r,
+                          double *__restrict__ rhat, const int4 *__restrict__ nbr, int nrows,
+                          const StepFactors *__restrict__ sf, KrylovState *st, double *partials, unsigned int *counter,
+                          Comm comm, unsigned long long loop_handle) {
+  __shared__ __align__(16) double s_scr[WPB * ROWS_SCRATCH];
+  const double fac = sf->rhs_fac;
+  double sums[2] = {0, 0}; // |r|^2, sum x0 (= +0)
+  double mx = 0;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double *sw = s_scr + warp * ROWS_SCRATCH;
+  for (int row0 = (blockIdx.x * WPB + warp) * 32; row0 < nrows; row0 += gridDim.x * WPB * 32) {
+    const int nv = min(32, nrows - row0);
+    double bb[8];
+    rhs_rows<HAS_UDEF>(vel, udef, chi, pold, nbr, row0, nv, fac, sw, lane, bb);
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      sums[0] = fma(bb[i], bb[i], sums[0]);
+      mx = fmax(mx, fabs(bb[i]));
+    }
+    double2 cb[4];
+    rows_to_chunk(sw, lane, bb, cb);
+    chunk_st(r, row0, nv, lane, cb);
+    chunk_st(rhat, row0, nv, lane, cb);
+    const double2 zero[4] = {};
+    chunk_st(x, row0, nv, lane, zero);
+  }
   grid_reduce<2, NT>(sums, mx, partials, counter, comm, [=](const double *t, double m) {
-    st->err = st->err_init = st->err_opt = m; // cuda.cu:428-430
-    st->xsum = t[1];
-    st->nrh2 = t[0];
-    st->iter = 0;
-    if (st->max_iter <= 0) st->done = 1;
-    prepare_iteration(st, t[0], t[0]);
-    set_loop_condition(loop_handle, st);
+    start_of_solve(st, t, m, loop_handle);
+    st->x0_zero = 1;
   });
 }
 
@@ -585,7 +628,9 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
   double sums[2] = {0, 0};
   // r^ of the interior blocks is needed only after the preconditioner: it is copied into a stage when the tile starts, so
   // its load overlaps the preconditioner and the stencil.  Two stages, alternating by tile: a copy is issued only after the
-  // CTA barriers of the tile that read the stage last.
+  // CTA barriers of the tile that read the stage last.  Iteration 0 and a restart read no r^: it equals r bit for bit (the
+  // start kernel stored r^ = r; a restart stores it here).
+  const bool rhat_is_r = restart || first;
   __shared__ __align__(16) double2 s_rhat[2 * 4 * 128];
   int par = 0;
   TILE_LOOP() {
@@ -594,10 +639,10 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
 #pragma unroll
     for (int j = 0; j < 4; j++) sl[j] = ts[4 * warp + j];
     double2 *stg = s_rhat + (par * 4 + (warp & 3)) * 128;
-    if (warp < 4 && !restart) blocks_stage(stg, rhat, sl, lane);
+    if (warp < 4 && !rhat_is_r) blocks_stage(stg, rhat, sl, lane);
     double2 cp[4], cr[4], ch[4];
     blocks_ld(r, sl, lane, cr);
-    if (restart || first) { // p = r, as in k_pupdate
+    if (rhat_is_r) { // p = r, as in k_pupdate
 #pragma unroll
       for (int j = 0; j < 4; j++) cp[j] = ch[j] = cr[j];
       if (restart && warp < 4) blocks_st(rhat, sl, lane, cr);
@@ -617,7 +662,7 @@ k_p_spmv(const double *__restrict__ r, double *__restrict__ rhat, double *p0, do
     double2 ca[4];
     tile_precond_lap(v, s_tile, sw, lane, warp, ts, ca);
     if (warp < 4) {
-      if (!restart) { // held in registers across the preconditioner it would cost spills
+      if (!rhat_is_r) { // held in registers across the preconditioner it would cost spills
         stage_wait();
         blocks_unstage(stg, sl, lane, ch);
       }
@@ -693,7 +738,7 @@ k_r_spmv(const double *__restrict__ r, const double *nu0, const double *nu1, dou
 // read from the plane (rows 1..32, chunk layout).  The plane is overwritten only after the next tile's first CTA barrier,
 // which every warp reaches after it has finished this tile.  When the tile starts, warps 0-3 copy r^ into a stage (as
 // k_p_spmv does) and keep r' in registers, and warps 4-7 keep p'; x is loaded after the stencil: held across the tile
-// with the others it would cost spills.
+// with the others it would cost spills.  Iteration 0 of a solve that started from x0 = +0 (a time step's) loads no x.
 __global__ void __launch_bounds__(NT, KTILE_CTAS)
 k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1, double *__restrict__ r,
           const double *__restrict__ rp, const double *__restrict__ rhat, const int *__restrict__ tiles, int ntiles,
@@ -704,6 +749,7 @@ k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1
   const double *xc = cur == 0 ? x0 : (cur == 1 ? x1 : x2);
   double *xn = nxt == 0 ? x0 : (nxt == 1 ? x1 : x2);
   const double *__restrict__ p = pair_in(st) ? p0 : p1; // what k_p_spmv of this iteration wrote
+  const bool x_zero = st->x0_zero && st->iter == 0;
   double sums[3] = {0, 0, 0}; // rhat.r, r.r, sum x
   double mx = 0;
   __shared__ __align__(16) double2 s_rhat[2 * 4 * 128]; // two stages, alternating by tile (see k_p_spmv)
@@ -747,7 +793,12 @@ k_x_final(double *x0, double *x1, double *x2, const double *p0, const double *p1
       blocks_st(r, sl, lane, ca);
     } else {
       double2 cx[4];
-      blocks_ld(xc, il, lane, cx);
+      if (x_zero) {
+#pragma unroll
+        for (int j = 0; j < 4; j++) cx[j] = make_double2(0.0, 0.0);
+      } else {
+        blocks_ld(xc, il, lane, cx);
+      }
       chunk_to_rows(sw, lane, ca, v);
       precond_row(v, sw, lane);
       rows_to_chunk(sw, lane, v, ca); // z_p
@@ -785,9 +836,8 @@ static PushView make_push(const cup2d_sim *s, int peer_index) {
   return pv;
 }
 
-// Start of a solve: Krylov state, r = b - A x0 (b = tmp, x0 = pres).  x0_halo_current: the halo slots of pres already
-// hold what the neighbours have (the step's right-hand-side kernel zeroes pres, halo slots included), so no refresh.
-int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current) {
+// Start of a solve: Krylov state, r = b - A x0 (b = tmp, x0 = pres)
+int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter) {
   int rc = g_consts.run(s->device, upload_consts);
   if (rc) return rc;
   const int nrows = (int)s->nloc * 8;
@@ -795,7 +845,7 @@ int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts
   const int4 *nbr = reinterpret_cast<const int4 *>(s->d_nbr);
   const bool has_irr = s->n_irr_rows > 0; // general rows present: kernels with the CSR override compiled in
   k_state_init<<<1, 1, 0, s->stream>>>(s->d_state, tol_abs, tol_rel, max_restarts, max_iter);
-  if (s->nranks > 1 && !x0_halo_current && (rc = halo_exchange_ptr(s, s->f[CUP2D_PRES], 1, CUP2D_PRES))) return rc;
+  if (s->nranks > 1 && (rc = halo_exchange_ptr(s, s->f[CUP2D_PRES], 1, CUP2D_PRES))) return rc;
   {
     ProfScope prof(s, KC_KINIT);
     if (has_irr)
@@ -806,6 +856,32 @@ int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts
       k_init<false><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_TMP], s->f[CUP2D_PRES], s->kx[0], s->kr, s->krhat, nbr,
                                                 nrows, s->d_state, s->d_partials, s->d_counter,
                                                 s->comm, irr_view(s), s->cond_handle);
+  }
+  s->launches += 2;
+  CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
+}
+
+// Start of a time step's solve: Krylov state, then b from the step's right-hand side, r = rhat = b and x = 0 in one kernel
+// (x0 = 0: no halo of it is needed).  pres is neither read nor written: the correction writes it.
+int poisson_begin_rhs(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, const StepRhs &rhs) {
+  int rc = g_consts.run(s->device, upload_consts);
+  if (rc) return rc;
+  const int nrows = (int)s->nloc * 8;
+  const int grid = red_grid(s, nrows);
+  const int4 *nbr = reinterpret_cast<const int4 *>(s->d_nbr);
+  k_state_init<<<1, 1, 0, s->stream>>>(s->d_state, tol_abs, tol_rel, max_restarts, max_iter);
+  if ((rc = pressure_rhs_inputs(s, rhs.has_udef))) return rc;
+  {
+    ProfScope prof(s, KC_RHS_START);
+    if (rhs.has_udef)
+      pressure_rhs_start_kernel<true><<<grid, NT, 0, s->stream>>>(
+          s->f[CUP2D_VEL], s->f[CUP2D_TMPV], s->f[CUP2D_CHI], s->f[CUP2D_POLD], s->kx[0], s->kr, s->krhat, nbr, nrows, rhs.dev,
+          s->d_state, s->d_partials, s->d_counter, s->comm, s->cond_handle);
+    else // no bodies: chi * div(udef) is identically zero (main.cpp:6980-6983 leaves tmpV = 0)
+      pressure_rhs_start_kernel<false><<<grid, NT, 0, s->stream>>>(
+          s->f[CUP2D_VEL], s->f[CUP2D_TMPV], s->f[CUP2D_CHI], s->f[CUP2D_POLD], s->kx[0], s->kr, s->krhat, nbr, nrows, rhs.dev,
+          s->d_state, s->d_partials, s->d_counter, s->comm, s->cond_handle);
   }
   s->launches += 2;
   CUP2D_CUDA(cudaGetLastError());
@@ -905,9 +981,8 @@ int poisson_result(cup2d_sim *s, int *iters, double *err) {
   return comm_check(s);
 }
 
-int poisson_solve(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter,
-                  int *iters, double *err, bool x0_halo_current) {
-  int rc = poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter, x0_halo_current);
+int poisson_solve(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, int *iters, double *err) {
+  int rc = poisson_begin(s, tol_abs, tol_rel, max_restarts, max_iter);
   if (rc) return rc;
   // fixed work (tolerances 0: the reference's first ten steps, main.cpp:7028-7030): everything is queued at once;
   // tolerance-driven: the host looks at the device's `done` flag every 8 iterations

@@ -6,7 +6,7 @@
 // scratch (rows.cuh).  Neighbour BLOCKS come through d_nbr[slot] = (W,E,S,N), -1 = domain wall, which
 // replaces the reference's BlockLab assembly (main.cpp:2270-2440) and ghost fill (main.cpp:3131-3154,
 // 3210-3245).
-#include "rows.cuh"
+#include "rhs.cuh"
 #include "sim.h"
 
 namespace cup2d {
@@ -75,99 +75,22 @@ int launch_umax(cup2d_sim *s, double *umax_out) {
   return CUP2D_OK;
 }
 
-// ------------------------------------------------------------------------------------------------
-// undivided divergence of a vector field on the warp's 32 rows, free-slip ghosts at walls
-// (pressure_rhs main.cpp:6105-6139: ((u_E - u_W) + v_N) - v_S, left to right; VectorLab ghosts
-// main.cpp:3131-3154: normal component negated)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void rows_div(const double2 (&cf)[8], const double *__restrict__ f, int nvalid,
-                                         const int4 nb, int slot, int y, double *sw, int lane,
-                                         double (&d)[8]) {
-  double2 c[8];
-  chunk2_to_rows(sw, nvalid, lane, cf, c);
-  if (lane < nvalid) {
-    const double2 *f2 = reinterpret_cast<const double2 *>(f);
-    double vu[8], vd[8];
-    {
-      double2 t[8];
-      if (y < 7) {
-        rows_peek2(sw, lane + 1, t);
-#pragma unroll
-        for (int i = 0; i < 8; i++) vu[i] = t[i].y;
-      } else if (nb.w >= 0) {
-        grow_load2(f, nb.w, 0, t);
-#pragma unroll
-        for (int i = 0; i < 8; i++) vu[i] = t[i].y;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; i++) vu[i] = -c[i].y;
-      }
-      if (y > 0) {
-        rows_peek2(sw, lane - 1, t);
-#pragma unroll
-        for (int i = 0; i < 8; i++) vd[i] = t[i].y;
-      } else if (nb.z >= 0) {
-        grow_load2(f, nb.z, 7, t);
-#pragma unroll
-        for (int i = 0; i < 8; i++) vd[i] = t[i].y;
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; i++) vd[i] = -c[i].y;
-      }
-    }
-    const double uW = nb.x >= 0 ? f2[(size_t)nb.x * 64 + y * 8 + 7].x : -c[0].x;
-    const double uE = nb.y >= 0 ? f2[(size_t)nb.y * 64 + y * 8 + 0].x : -c[7].x;
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-      const double e = i < 7 ? c[i + 1].x : uE;
-      const double w = i > 0 ? c[i - 1].x : uW;
-      d[i] = ((e - w) + vu[i]) - vd[i];
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; i++) d[i] = 0.0;
-  }
-}
-
 // tmp = fac*(div vel) - fac*chi*(div udef) - lap(pold);  pres = 0     (main.cpp:7011-7027)
+// The stand-alone form (cup2d_pressure_rhs): a time step forms the same b in pressure_rhs_start_kernel (poisson.cu) and
+// starts its solve there instead.
 template <bool HAS_UDEF>
 __global__ void __launch_bounds__(NT)
 pressure_rhs_kernel(const double *__restrict__ vel, const double *__restrict__ udef,
                     const double *__restrict__ chi, const double *__restrict__ pold,
                     double *__restrict__ tmp, double *__restrict__ pres, const int4 *__restrict__ nbr,
-                    int nrows, double fac_arg, const StepFactors *__restrict__ sf, int nrows_zero) {
+                    int nrows, double fac) {
   __shared__ __align__(16) double s_scr[WPB * ROWS_SCRATCH];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   double *sw = s_scr + warp * ROWS_SCRATCH;
-  const double fac = sf ? sf->rhs_fac : fac_arg;
-  // pres = 0 on the halo slots as well (rows nrows .. nrows_zero): the solve that follows starts from x0 = pres and
-  // then needs no halo refresh of it
-  for (int i = nrows * 4 + blockIdx.x * NT + threadIdx.x; i < nrows_zero * 4; i += gridDim.x * NT)
-    reinterpret_cast<double2 *>(pres)[i] = make_double2(0.0, 0.0);
   for (int row0 = (blockIdx.x * WPB + warp) * 32; row0 < nrows; row0 += gridDim.x * WPB * 32) {
     const int nv = min(32, nrows - row0);
-    const int row = row0 + lane, slot = row >> 3, y = row & 7;
-    const int4 nb = lane < nv ? nbr[slot] : make_int4(-1, -1, -1, -1);
-    double out[8], t[8], pc[8];
-    // every global load of the chunk is issued up front (memory-level parallelism), then the smem work
-    double2 cvel[8], cpold[4];
-    chunk2_ld(vel, row0, nv, lane, cvel);
-    chunk_ld(pold, row0, nv, lane, cpold);
-    rows_div(cvel, vel, nv, nb, slot, y, sw, lane, out);
-#pragma unroll
-    for (int i = 0; i < 8; i++) out[i] *= fac;
-    if (HAS_UDEF) {
-      double du[8];
-      double2 cud[8];
-      chunk2_ld(udef, row0, nv, lane, cud);
-      rows_div(cud, udef, nv, nb, slot, y, sw, lane, du);
-      rows_load1(chi, row0, nv, sw, lane, t);
-#pragma unroll
-      for (int i = 0; i < 8; i++) out[i] = out[i] - fac * t[i] * du[i];
-    }
-    rows_lap_c(cpold, pold, row0, nv, nbr, sw, lane, pc, t);
-#pragma unroll
-    for (int i = 0; i < 8; i++) out[i] -= t[i];
+    double out[8];
+    rhs_rows<HAS_UDEF>(vel, udef, chi, pold, nbr, row0, nv, fac, sw, lane, out);
     rows_store1(tmp, row0, nv, sw, lane, out);
 #pragma unroll
     for (int i = 0; i < 8; i++) out[i] = 0.0;
@@ -175,8 +98,8 @@ pressure_rhs_kernel(const double *__restrict__ vel, const double *__restrict__ u
   }
 }
 
-int launch_pressure_rhs(cup2d_sim *s, double dt, bool has_udef, const StepFactors *dev, bool zero_pres_halo) {
-  // pold <- pres is a pointer swap; the kernel then zeroes the new pres (main.cpp:7016-7021)
+int pressure_rhs_inputs(cup2d_sim *s, bool has_udef) {
+  // pold <- pres is a pointer swap; the right-hand side then reads pold (main.cpp:7016-7021)
   swap_fields(s, CUP2D_PRES, CUP2D_POLD);
   if (s->nranks > 1) {
     int rc;
@@ -184,19 +107,24 @@ int launch_pressure_rhs(cup2d_sim *s, double dt, bool has_udef, const StepFactor
     if (has_udef && (rc = halo_exchange_ptr(s, s->f[CUP2D_TMPV], 2, CUP2D_TMPV))) return rc;
     if ((rc = halo_exchange_ptr(s, s->f[CUP2D_POLD], 1, CUP2D_POLD))) return rc;
   }
+  return CUP2D_OK;
+}
+
+int launch_pressure_rhs(cup2d_sim *s, double dt, bool has_udef) {
+  int rc = pressure_rhs_inputs(s, has_udef);
+  if (rc) return rc;
   const int nrows = (int)s->nloc * 8;
   const int grid = min((nrows + NT - 1) / NT, s->num_sms * 8);
   const double fac = 0.5 * s->h / dt; // main.cpp:6119
-  const int nrows_zero = zero_pres_halo ? (int)s->nslots * 8 : nrows;
   ProfScope prof(s, KC_RHS);
   if (has_udef)
     pressure_rhs_kernel<true><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_VEL], s->f[CUP2D_TMPV], s->f[CUP2D_CHI],
                                                           s->f[CUP2D_POLD], s->f[CUP2D_TMP], s->f[CUP2D_PRES],
-                                                          reinterpret_cast<const int4 *>(s->d_nbr), nrows, fac, dev, nrows_zero);
+                                                          reinterpret_cast<const int4 *>(s->d_nbr), nrows, fac);
   else // no bodies: chi * div(udef) is identically zero (main.cpp:6980-6983 leaves tmpV = 0)
     pressure_rhs_kernel<false><<<grid, NT, 0, s->stream>>>(s->f[CUP2D_VEL], s->f[CUP2D_TMPV], s->f[CUP2D_CHI],
                                                            s->f[CUP2D_POLD], s->f[CUP2D_TMP], s->f[CUP2D_PRES],
-                                                           reinterpret_cast<const int4 *>(s->d_nbr), nrows, fac, dev, nrows_zero);
+                                                           reinterpret_cast<const int4 *>(s->d_nbr), nrows, fac);
   s->launches++;
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;

@@ -41,7 +41,7 @@ struct KrylovState {
   int done;                                // 1: stop (converged / restart cap / max_iter)
   int restart_now;                         // 1: next p-update performs the restart of cuda.cu:457-477
   int cur, opt;                            // which of the 3 x buffers holds x / x_opt
-  int pad;
+  int x0_zero;                             // 1: the solve started from x0 = +0 (x of iteration 0 need not be read)
 };
 
 // dt-dependent factors of the current time step, device-resident (k_step_factors): a step captured in a CUDA graph
@@ -153,7 +153,7 @@ struct cup2d_sim {
 
 namespace cup2d {
 enum KClass { KC_ADVECT = 0, KC_UMAX, KC_RHS, KC_CORRECT, KC_KINIT, KC_PUPDATE, KC_SPMV_NU, KC_XRUPDATE,
-              KC_SPMV_T, KC_FINAL, KC_P_SPMV, KC_R_SPMV, KC_X_FINAL, KC_HALO, KC_VORT, KC_COUNT };
+              KC_SPMV_T, KC_FINAL, KC_P_SPMV, KC_R_SPMV, KC_X_FINAL, KC_HALO, KC_VORT, KC_RHS_START, KC_COUNT };
 // bracket one launch with events when profiling is on (no-op otherwise)
 struct ProfScope {
   cup2d_sim *s;
@@ -191,7 +191,8 @@ int launch_advect(cup2d_sim *s, const double *in, const double *old, double *out
 int launch_umax(cup2d_sim *s, double *umax_out);
 int launch_umax_async(cup2d_sim *s);                      // umax -> d_scal[0], no host synchronisation
 int launch_step_factors(cup2d_sim *s, double dt_host);    // d_fac from dt_host (> 0) or from d_scal[0] (the dt rule on the device)
-int launch_pressure_rhs(cup2d_sim *s, double dt, bool has_udef, const StepFactors *dev = nullptr, bool zero_pres_halo = false);
+int launch_pressure_rhs(cup2d_sim *s, double dt, bool has_udef); // tmp = b, pres = 0 (cup2d_pressure_rhs)
+int pressure_rhs_inputs(cup2d_sim *s, bool has_udef);              // pold <- pres, halo refreshes of vel, tmpV, pold
 int launch_pressure_correct(cup2d_sim *s, double dt, const StepFactors *dev = nullptr, bool pold_halo_current = false);
 int launch_adapt_tags(cup2d_sim *s, double rtol, int chi_cells, double *linf_host);
 int dump_fields(cup2d_sim *s, double time, const char *path);
@@ -202,14 +203,20 @@ int shape_integrals(cup2d_sim *s, int shape, double lambda, double dt, double cx
 int shape_penalize(cup2d_sim *s, int shape, double lambda, double dt, double cx, double cy, double us, double vs,
                    double omega);
 int udef_assemble(cup2d_sim *s);
-int poisson_solve(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter,
-                  int *iters, double *err, bool x0_halo_current = false);
-int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current);
+int poisson_solve(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, int *iters, double *err);
+int poisson_begin(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter);
+// The right-hand side of a time step (vel, tmpV = u_def if has_udef, chi, pold; factor from dev) as the start of its solve
+struct StepRhs {
+  bool has_udef;
+  const StepFactors *dev;
+};
+int poisson_begin_rhs(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, const StepRhs &rhs);
 int poisson_iterations(cup2d_sim *s, int n, cudaStream_t stream);
 int poisson_result(cup2d_sim *s, int *iters, double *err);
-// begin + iterations of an enqueued solve (csrc/api.cu): a WHILE node while capturing a tolerance-driven solve, else launches
-int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool x0_halo_current,
-                    bool capturing);
+// begin + iterations of an enqueued solve (csrc/api.cu): a WHILE node while capturing a tolerance-driven solve, else launches.
+// rhs: start from a time step's right-hand side (poisson_begin_rhs); null: from b = tmp and x0 = pres (poisson_begin)
+int poisson_enqueue(cup2d_sim *s, double tol_abs, double tol_rel, int max_restarts, int max_iter, bool capturing,
+                    const StepRhs *rhs = nullptr);
 int halo_exchange_ptr(cup2d_sim *s, double *base, int dim, int peer_index, bool done_barrier = true);
 int halo_exchange_xopt(cup2d_sim *s); // halo of the x buffer KrylovState::opt names (chosen on the device)
 int comm_check(cup2d_sim *s);         // CUP2D_ECOMM if a cross-GPU wait of this rank was given up

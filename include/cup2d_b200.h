@@ -137,7 +137,9 @@ int cup2d_penalize(cup2d_sim *s, int shape, double lambda, double dt, double cx,
  * the u_def input of cup2d_pressure_rhs.  Bit-identical to the reference. */
 int cup2d_udef_assemble(cup2d_sim *s);
 /* One full time step of the hot path (no bodies): compute_dt (unless dt>0 is given), rk2, tmpV=0
- * (or kept if keep_udef), pressure_rhs, poisson_solve, pressure_correct.  Returns dt used. */
+ * (or kept if keep_udef), pressure_rhs, poisson_solve, pressure_correct.  Returns dt used.  vel, pres and pold come out
+ * as from that sequence of calls, but the solve starts in the right-hand-side kernel: after a step, tmp does NOT hold the
+ * right-hand side (call cup2d_pressure_rhs to get it there). */
 int cup2d_step(cup2d_sim *s, double dt_in, int keep_udef, double tol_abs, double tol_rel,
                int max_restarts, int max_iter, double *dt_out, int *iters_out, double *err_out);
 /* The same step, asynchronously: cup2d_step_enqueue puts the whole step on the context's stream and returns without
