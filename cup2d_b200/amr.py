@@ -120,6 +120,7 @@ class AmrSimulation:
         self.lib = _l.load_library()
         self.blocks = np.ascontiguousarray(level_ij, dtype=np.int32).reshape(-1, 3)
         self.bpdx, self.bpdy = int(bpdx), int(bpdy)
+        self._rank = None   # distributed contexts: this rank
         self._h = C.c_void_p()
         _l.check(self.lib.cup2d_amr_create(len(self.blocks), self.blocks.ctypes.data_as(C.POINTER(C.c_int32)), bpdx, bpdy,
                                            float(h0), float(nu), device, C.byref(self._h)))
@@ -134,10 +135,16 @@ class AmrSimulation:
         rb = np.ascontiguousarray(rank_begin, dtype=np.int64)
         nranks = len(rb) - 1
         self.blocks = allb[int(rb[rank]):int(rb[rank + 1])]
+        self._rank = int(rank)
         self.bpdx, self.bpdy = int(bpdx), int(bpdy)
         self._h = C.c_void_p()
         _l.check(self.lib.cup2d_amr_create_ranks(len(allb), allb.ctypes.data_as(C.POINTER(C.c_int32)), bpdx, bpdy, float(h0), float(nu),
                                                  int(rank), nranks, rb.ctypes.data_as(C.POINTER(C.c_int64)), device, C.byref(self._h)))
+        self._attach_peers(nranks, dist)
+        return self
+
+    def _attach_peers(self, nranks, dist):
+        """export this rank's peer blob, all-gather the ranks' blobs over `dist` and map the peers (cup2d_amr_peer_attach)"""
         n = self.lib.cup2d_peer_blob_size()
         blob = (C.c_ubyte * n)()
         _l.check(self.lib.cup2d_amr_peer_export(self._h, blob))
@@ -149,7 +156,26 @@ class AmrSimulation:
         _l.check(self.lib.cup2d_amr_peer_attach(self._h, (C.c_ubyte * len(allblob)).from_buffer_copy(allblob)))
         if dist is not None and nranks > 1:
             dist.barrier()
-        return self
+
+    def rank_begin(self):
+        """the partition of the block list, rank_begin[nranks+1] (cup2d_amr_rank_begin); [0, nb] for a plain context"""
+        n = self.lib.cup2d_amr_rank_begin(self._h, None)
+        if n < 0:
+            _l.check(int(n))
+        out = np.empty(n + 1, dtype=np.int64)
+        self.lib.cup2d_amr_rank_begin(self._h, out.ctypes.data_as(C.POINTER(C.c_int64)))
+        return out
+
+    def _after_regrid(self, changed, dist):
+        """on a distributed context: re-attach the peers after a change with several ranks, this rank's new range in blocks"""
+        allb = self.block_list()
+        if self._rank is None:
+            self.blocks = allb
+            return
+        rb = self.rank_begin()
+        if len(rb) > 2 and changed:
+            self._attach_peers(len(rb) - 1, dist)
+        self.blocks = allb[int(rb[self._rank]):int(rb[self._rank + 1])]
 
     def upload(self, name, blocks):
         a = np.ascontiguousarray(blocks, dtype=np.float64)
@@ -257,17 +283,22 @@ class AmrSimulation:
         _l.check(self.lib.cup2d_amr_adapt_tags(self._h, float(rtol), int(level_max), out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
-    def regrid(self, new_blocks):
+    def regrid(self, new_blocks, dist=None):
         """move the context onto `new_blocks` (one refine / compress step away, e.g. from adapt_mesh) with adapt()'s field
-        transfer on the device (cup2d_amr_regrid); tmpV is zero afterwards and the shapes have to be set again"""
+        transfer on the device (cup2d_amr_regrid); tmpV is zero afterwards and the shapes have to be set again.  On a
+        distributed context every rank passes the whole new list; the ranks move onto the reference's new partition, `dist`
+        re-attaches the peers, and `blocks` becomes this rank's new range"""
         b = np.ascontiguousarray(new_blocks, dtype=np.int32).reshape(-1, 3)
+        before = None if self._rank is None else (self.block_list(), self.rank_begin())
         _l.check(self.lib.cup2d_amr_regrid(self._h, len(b), b.ctypes.data_as(C.POINTER(C.c_int32))))
-        self.blocks = b.copy()
+        changed = before is not None and not (np.array_equal(before[0], b) and np.array_equal(before[1], self.rank_begin()))
+        self._after_regrid(changed, dist)
 
-    def adapt(self, rtol, ctol, level_max, block_linf=None):
+    def adapt(self, rtol, ctol, level_max, block_linf=None, dist=None):
         """adapt() on the device-resident fields in one call (cup2d_amr_adapt): tags (or the caller's per-block `block_linf`),
         decision, order and transfer on the device, the same mesh and fields as adapt_tags -> adapt_mesh -> regrid; returns
-        whether the mesh changed"""
+        whether the mesh changed (on a distributed context: the mesh or the partition, and `block_linf` holds this rank's
+        blocks; `dist` re-attaches the peers and `blocks` becomes this rank's new range)"""
         linf = None
         if block_linf is not None:
             linf = np.ascontiguousarray(block_linf, dtype=np.float64)
@@ -275,7 +306,7 @@ class AmrSimulation:
         changed = C.c_int32()
         _l.check(self.lib.cup2d_amr_adapt(self._h, None if linf is None else linf.ctypes.data_as(C.POINTER(C.c_double)),
                                           float(rtol), float(ctol), int(level_max), None, C.byref(changed)))
-        self.blocks = self.block_list()
+        self._after_regrid(bool(changed.value), dist)
         return bool(changed.value)
 
     def block_list(self):

@@ -589,6 +589,10 @@ __global__ void amr_allreduce_kernel(double *v, Comm comm) {
 static int dist_allreduce(cup2d_amr *a, double &s0, double &s1, double &mx) {
   if (!a->dist || a->nranks == 1) return CUP2D_OK;
   cup2d_sim *ps = a->poisson;
+  if (!ps->peers_attached) { // e.g. between a regrid onto new arrays and the re-attach
+    set_error("distributed context: all-reduce before cup2d_amr_peer_attach");
+    return CUP2D_ESTATE;
+  }
   ps->h_scal[0] = s0, ps->h_scal[1] = s1, ps->h_scal[2] = mx;
   CUP2D_CUDA(cudaMemcpyAsync(ps->d_scal, ps->h_scal, 3 * sizeof(double), cudaMemcpyHostToDevice, a->stream));
   amr_allreduce_kernel<<<1, 32, 0, a->stream>>>(ps->d_scal, ps->comm);

@@ -17,6 +17,7 @@
 // the transfer's), and feeds the same transfer (regrid_apply) from the device without cup2d_amr_regrid's host classification.
 #include "sim.h"
 #include <algorithm>
+#include <cstring>
 #include <array>
 #include <map>
 #include <string>
@@ -64,6 +65,17 @@ __global__ void amr_regrid_copy_kernel(RgFields F, const int2 *__restrict__ pair
   }
 }
 
+// one value of a compressed parent: the average of the 2x2 cells (i, j) .. (i+1, j+1), component d, of child block b
+__device__ __forceinline__ double rg_average4(const double *b, int dim, int i, int j, int d) {
+  const double v00 = b[dim * (8 * j + i) + d], v01 = b[dim * (8 * (j + 1) + i) + d];
+  const double v10 = b[dim * (8 * j + i + 1) + d], v11 = b[dim * (8 * (j + 1) + i + 1) + d];
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(add_rn(add_rn(add_rn(v00, v01), v10), v11), 4.0);
+#else
+  return (((v00 + v01) + v10) + v11) / 4;
+#endif
+}
+
 // compressed groups: children[4] (J*2 + I order) -> new block; one thread per output value of every transferred field
 __global__ void amr_regrid_compress_kernel(RgFields F, const int *__restrict__ dst, const int4 *__restrict__ kids, int64_t ngroups) {
   const int per = 2 * F.off2[RG_NF]; // doubles of one block over the fields
@@ -76,14 +88,7 @@ __global__ void amr_regrid_compress_kernel(RgFields F, const int *__restrict__ d
     const int4 k4 = kids[q];
     const int I = ox >> 2, J = oy >> 2, kid = J == 0 ? (I == 0 ? k4.x : k4.y) : (I == 0 ? k4.z : k4.w);
     const int i = 2 * (ox & 3), j = 2 * (oy & 3);
-    const double *b = F.src[f] + (int64_t)kid * 64 * dim;
-    const double v00 = b[dim * (8 * j + i) + d], v01 = b[dim * (8 * (j + 1) + i) + d];
-    const double v10 = b[dim * (8 * j + i + 1) + d], v11 = b[dim * (8 * (j + 1) + i + 1) + d];
-#ifdef __CUDA_ARCH__
-    F.dst[f][(int64_t)dst[q] * 64 * dim + s] = __ddiv_rn(add_rn(add_rn(add_rn(v00, v01), v10), v11), 4.0);
-#else
-    F.dst[f][(int64_t)dst[q] * 64 * dim + s] = (((v00 + v01) + v10) + v11) / 4;
-#endif
+    F.dst[f][(int64_t)dst[q] * 64 * dim + s] = rg_average4(F.src[f] + (int64_t)kid * 64 * dim, dim, i, j, d);
   }
 }
 
@@ -109,6 +114,25 @@ __global__ void amr_regrid_lab_kernel(RgFields F, RgLab L) {
   }
 }
 
+// the four cells of the 2x2 group (i, j) of child (I, J), component d, from the parent's lab um (main.cpp:5012-5028) into
+// the child's block b
+__device__ __forceinline__ void rg_refine_group(const double *um, double *b, int dim, int d, int I, int J, int i, int j) {
+  constexpr int nm = 10;
+  const int i0 = i / 2 + 4 * I + 1, j0 = j / 2 + 4 * J + 1, im = i0 - 1, ip = i0 + 1, jm = j0 - 1, jp = j0 + 1;
+  const double l00 = um[dim * (nm * j0 + i0) + d], l0p = um[dim * (nm * jp + i0) + d], lm0 = um[dim * (nm * j0 + im) + d];
+  const double lmm = um[dim * (nm * jm + im) + d], lmp = um[dim * (nm * jp + im) + d], lp0 = um[dim * (nm * j0 + ip) + d];
+  const double lpm = um[dim * (nm * jm + ip) + d], lpp = um[dim * (nm * jp + ip) + d], l0m = um[dim * (nm * jm + i0) + d];
+  const double x = mul_rn(0.5, add_rn(lp0, -lm0)), y = mul_rn(0.5, add_rn(l0p, -l0m));
+  const double x2 = add_rn(add_rn(lp0, lm0), -mul_rn(2.0, l00)), y2 = add_rn(add_rn(l0p, l0m), -mul_rn(2.0, l00));
+  const double xy = mul_rn(0.25, add_rn(add_rn(lpp, lmm), -add_rn(lpm, lmp)));
+  const double c = add_rn(mul_rn(0.03125, x2), mul_rn(0.03125, y2)), e = mul_rn(0.0625, xy);
+  const double ax = mul_rn(0.25, x), ay = mul_rn(0.25, y);
+  b[dim * (8 * j + i) + d] = add_rn(add_rn(l00, add_rn(mul_rn(-0.25, x), -ay)), add_rn(c, e));
+  b[dim * (8 * j + i + 1) + d] = add_rn(add_rn(l00, add_rn(ax, -ay)), add_rn(c, -e));
+  b[dim * (8 * (j + 1) + i) + d] = add_rn(add_rn(l00, add_rn(mul_rn(-0.25, x), ay)), add_rn(c, -e));
+  b[dim * (8 * (j + 1) + i + 1) + d] = add_rn(add_rn(l00, add_rn(ax, ay)), add_rn(c, e));
+}
+
 // children of the refined parents from their labs (main.cpp:4982-5031): one thread per (parent, field, child, 2x2 group,
 // component) evaluates the four cells of its group.  child_dst[4 q + J*2 + I] = new block of child (I, J) of parent q.
 __global__ void amr_regrid_refine_kernel(RgFields F, RgLab L, const int *__restrict__ child_dst, int64_t nparents) {
@@ -119,24 +143,82 @@ __global__ void amr_regrid_refine_kernel(RgFields F, RgLab L, const int *__restr
     while (s >= 2 * F.off2[f + 1]) f++;
     s -= 2 * F.off2[f];
     const int dim = F.dim[f], d = s % dim, g = s / dim, child = g >> 4, gi = g & 3, gj = (g >> 2) & 3;
-    const double *um0 = L.lab[f];
-    const int I = child & 1, J = child >> 1, i = 2 * gi, j = 2 * gj;
-    const double *um = um0 + q * 100 * dim;
-    constexpr int nm = 10;
-    const int i0 = i / 2 + 4 * I + 1, j0 = j / 2 + 4 * J + 1, im = i0 - 1, ip = i0 + 1, jm = j0 - 1, jp = j0 + 1;
-    const double l00 = um[dim * (nm * j0 + i0) + d], l0p = um[dim * (nm * jp + i0) + d], lm0 = um[dim * (nm * j0 + im) + d];
-    const double lmm = um[dim * (nm * jm + im) + d], lmp = um[dim * (nm * jp + im) + d], lp0 = um[dim * (nm * j0 + ip) + d];
-    const double lpm = um[dim * (nm * jm + ip) + d], lpp = um[dim * (nm * jp + ip) + d], l0m = um[dim * (nm * jm + i0) + d];
-    const double x = mul_rn(0.5, add_rn(lp0, -lm0)), y = mul_rn(0.5, add_rn(l0p, -l0m));
-    const double x2 = add_rn(add_rn(lp0, lm0), -mul_rn(2.0, l00)), y2 = add_rn(add_rn(l0p, l0m), -mul_rn(2.0, l00));
-    const double xy = mul_rn(0.25, add_rn(add_rn(lpp, lmm), -add_rn(lpm, lmp)));
-    const double c = add_rn(mul_rn(0.03125, x2), mul_rn(0.03125, y2)), e = mul_rn(0.0625, xy);
-    const double ax = mul_rn(0.25, x), ay = mul_rn(0.25, y);
-    double *b = F.dst[f] + (int64_t)child_dst[4 * q + child] * 64 * dim;
-    b[dim * (8 * j + i) + d] = add_rn(add_rn(l00, add_rn(mul_rn(-0.25, x), -ay)), add_rn(c, e));
-    b[dim * (8 * j + i + 1) + d] = add_rn(add_rn(l00, add_rn(ax, -ay)), add_rn(c, -e));
-    b[dim * (8 * (j + 1) + i) + d] = add_rn(add_rn(l00, add_rn(mul_rn(-0.25, x), ay)), add_rn(c, -e));
-    b[dim * (8 * (j + 1) + i + 1) + d] = add_rn(add_rn(l00, add_rn(ax, ay)), add_rn(c, e));
+    rg_refine_group(L.lab[f] + q * 100 * dim, F.dst[f] + (int64_t)child_dst[4 * q + child] * 64 * dim, dim, d, child & 1,
+                    child >> 1, 2 * gi, 2 * gj);
+  }
+}
+
+// ---- the same transfer on a distributed context (cup2d_amr_create_ranks) --------------------------------------------------
+// Every rank computes its own new blocks only and reads the old blocks wherever they live: old global block g is local
+// block g - rb[r] of rank r (the old partition), read through the peer mapping of rank r's field array.  Same arithmetic,
+// operand order and round-to-nearest operations as the one-rank kernels above, so the values are the same bits.
+struct RgPeer {
+  const double *base[RG_NF][MAX_RANKS]; // per field: every rank's old array as mapped here (this rank: its own)
+  int64_t rb[MAX_RANKS + 1];
+  int nranks;
+  __device__ __forceinline__ const double *block(int f, int64_t g, int dim) const {
+    int r = 0;
+    while (r + 1 < nranks && g >= rb[r + 1]) r++;
+    return base[f][r] + (g - rb[r]) * 64 * dim;
+  }
+};
+
+// (new local block, old global block) pairs
+__global__ void amr_regrid_peer_copy_kernel(RgFields F, RgPeer P, const int2 *__restrict__ pairs, int64_t npairs) {
+  const int per = F.off2[RG_NF];
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < npairs * per; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t q = t / per;
+    int s = (int)(t - q * per), f = 0;
+    while (s >= F.off2[f + 1]) f++;
+    s -= F.off2[f];
+    const int2 pr = pairs[q];
+    const int64_t n2 = 32 * F.dim[f];
+    reinterpret_cast<double2 *>(F.dst[f])[pr.x * n2 + s] = reinterpret_cast<const double2 *>(P.block(f, pr.y, F.dim[f]))[s];
+  }
+}
+
+// compressed groups: old global children -> new local block
+__global__ void amr_regrid_peer_compress_kernel(RgFields F, RgPeer P, const int *__restrict__ dst, const int4 *__restrict__ kids,
+                                                int64_t ngroups) {
+  const int per = 2 * F.off2[RG_NF];
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < ngroups * per; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t q = t / per;
+    int s = (int)(t - q * per), f = 0;
+    while (s >= 2 * F.off2[f + 1]) f++;
+    s -= 2 * F.off2[f];
+    const int dim = F.dim[f], d = s % dim, cell = s / dim, ox = cell & 7, oy = cell >> 3;
+    const int4 k4 = kids[q];
+    const int I = ox >> 2, J = oy >> 2, kid = J == 0 ? (I == 0 ? k4.x : k4.y) : (I == 0 ? k4.z : k4.w);
+    F.dst[f][(int64_t)dst[q] * 64 * dim + s] = rg_average4(P.block(f, kid, dim), dim, 2 * (ox & 3), 2 * (oy & 3), d);
+  }
+}
+
+// labs of the refined parents, sources named by old global block
+__global__ void amr_regrid_peer_lab_kernel(RgFields F, RgPeer P, RgLab L) {
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < L.rbeg[RG_NF]; t += (int64_t)gridDim.x * blockDim.x) {
+    int f = 0;
+    while (t >= L.rbeg[f + 1]) f++;
+    const int64_t r = t - L.rbeg[f];
+    const int dim = F.dim[f], k = dim == 2 ? 0 : 1;
+    double acc = 0.0;
+    for (int64_t e = L.rowptr[k][r]; e < L.rowptr[k][r + 1]; e++)
+      acc = add_rn(acc, mul_rn(L.w[k][e], P.block(f, L.sb[k][e], dim)[L.sc[k][e]]));
+    L.lab[f][r] = acc;
+  }
+}
+
+// children of the refined parents; child_dst = new local block, or -1 for a child another rank holds
+__global__ void amr_regrid_peer_refine_kernel(RgFields F, RgLab L, const int *__restrict__ child_dst, int64_t nparents) {
+  const int per = 2 * F.off2[RG_NF];
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < nparents * per; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t q = t / per;
+    int s = (int)(t - q * per), f = 0;
+    while (s >= 2 * F.off2[f + 1]) f++;
+    s -= 2 * F.off2[f];
+    const int dim = F.dim[f], d = s % dim, g = s / dim, child = g >> 4, gi = g & 3, gj = (g >> 2) & 3;
+    const int cd = child_dst[4 * q + child];
+    if (cd < 0) continue;
+    rg_refine_group(L.lab[f] + q * 100 * dim, F.dst[f] + (int64_t)cd * 64 * dim, dim, d, child & 1, child >> 1, 2 * gi, 2 * gj);
   }
 }
 
@@ -474,6 +556,201 @@ static int regrid_apply(cup2d_amr *a, const char *who, int64_t nnew, const int32
   return CUP2D_OK;
 }
 
+// ---- distributed contexts ------------------------------------------------------------------------------------------------
+// The whole adapt runs on every rank: the same arguments (checked), the same global tags (gathered over the peer mapping),
+// the same decision kernels over the whole list, the same new list and classification, the same new partition.  Then each
+// rank builds its share of the new mesh (cup2d_amr_create_ranks) and fills its own new blocks from the old blocks of
+// whichever rank holds them.  Three bounded peer barriers on the old context, all the all-reduce of amr_dist_sum_vec:
+// the argument check (for a regrid it also orders every rank's last writes of its old fields before the reads), the tags
+// (every rank's tags and old fields final before anyone reads them), and the end of the reads (before anyone frees the old
+// arrays).  A rank that never arrives makes the others return CUP2D_ECOMM instead of waiting.
+
+// The reference's new partition (main.cpp:5196-5205, 5332-5349) from the number of new blocks each rank produces (a copy:
+// the old block's owner; the children of a refined block: its owner; a compressed parent: the owner of its (even i, even j)
+// sibling, to which the reference moves the other three first).  Full rebalance if max / min > 1.01 or a rank produces none:
+// total / nranks each, the first total % nranks ranks one more.  Otherwise (n_r - n_{r+1}) / 4 blocks, C division truncating
+// toward zero, go from rank r to rank r+1 (a negative number the other way).  Returns the new rank_begin.
+static std::vector<int64_t> rebalance(const std::vector<int64_t> &n) {
+  const int W = (int)n.size();
+  int64_t total = 0, mx = n[0], mn = n[0];
+  for (int64_t v : n) total += v, mx = std::max(mx, v), mn = std::min(mn, v);
+  std::vector<int64_t> cnt(W), rb(W + 1, 0);
+  if (mn == 0 || (double)mx / (double)mn > 1.01) {
+    for (int r = 0; r < W; r++) cnt[r] = total / W + (r < total % W ? 1 : 0);
+  } else {
+    for (int r = 0; r < W; r++) {
+      const int64_t left = r == 0 ? 0 : (n[r] - n[r - 1]) / 4, right = r == W - 1 ? 0 : (n[r] - n[r + 1]) / 4;
+      cnt[r] = n[r] - left - right;
+    }
+  }
+  for (int r = 0; r < W; r++) rb[r + 1] = rb[r] + cnt[r];
+  return rb;
+}
+
+// owner rank of global block g under the partition rb
+static int owner_of(const std::vector<int64_t> &rb, int64_t g) {
+  return (int)(std::upper_bound(rb.begin(), rb.end(), g) - rb.begin()) - 1;
+}
+
+// one bounded all-rank barrier on the old context that also checks that every rank passed the same `mine` values (bitwise):
+// each rank contributes its row of an nranks x K table, the sum gives every rank every row
+static int dist_agree(cup2d_amr *a, const char *who, const std::vector<double> &mine) {
+  const int K = (int)mine.size(), W = a->nranks;
+  if (W == 1) return CUP2D_OK;
+  std::vector<double> v((size_t)W * K, 0.0);
+  std::copy(mine.begin(), mine.end(), v.begin() + (size_t)a->rank * K);
+  int rc = amr_dist_sum_vec(a, v.data(), W * K);
+  if (rc) return rc;
+  for (int r = 1; r < W; r++)
+    if (memcmp(v.data(), v.data() + (size_t)r * K, K * sizeof(double)) != 0) {
+      set_error(std::string(who) + ": the ranks passed different arguments");
+      return CUP2D_ECOMM;
+    }
+  return CUP2D_OK;
+}
+
+// 64-bit FNV-1a of a block list, as two doubles (exact: 32 bits each)
+static void list_hash(const int32_t *lij, int64_t n, std::vector<double> &out) {
+  u64 h = 1469598103934665603ull;
+  for (int64_t k = 0; k < 3 * n; k++) h = (h ^ (u64)(uint32_t)lij[k]) * 1099511628211ull;
+  out.push_back((double)(h >> 32));
+  out.push_back((double)(h & 0xffffffffull));
+}
+
+// The global classification of a regrid, on the host: copy pairs (new, old), compressed groups kids[g] -> cdst[g], refined
+// parents with child_dst[4 q + J*2 + I] (global block ids throughout).  Moves every rank of the distributed context `a` onto
+// its range of the new list under the reference's partition; no-op (changed = false) if neither list nor partition changes.
+struct RgPlanHost {
+  std::vector<int2> pairs;
+  std::vector<int4> kids;
+  std::vector<int32_t> cdst, parents, child_dst;
+};
+static int regrid_apply_dist(cup2d_amr *a, const char *who, int64_t nnew, const int32_t *new_level_ij, int bpdx, int bpdy,
+                             const RgPlanHost &C, bool *changed) {
+  const int W = a->nranks, me = a->rank;
+  const std::vector<int64_t> &orb = a->rank_begin;
+  std::vector<int64_t> produced(W, 0);
+  for (const int2 &p : C.pairs) produced[owner_of(orb, p.y)]++;
+  for (int32_t p : C.parents) produced[owner_of(orb, p)] += 4;
+  for (const int4 &k : C.kids) produced[owner_of(orb, k.x)]++;
+  const std::vector<int64_t> rb = rebalance(produced);
+  bool empty = false;
+  for (int r = 0; r < W; r++) empty |= rb[r + 1] <= rb[r];
+  int bx = 0, by = 0;
+  const std::vector<int> &old = amr_plan_level_ij(a->plan, &bx, &by);
+  *changed = !(nnew == a->nglobal && std::equal(old.begin(), old.end(), new_level_ij) && rb == orb);
+  if (empty || !*changed) { // every rank takes this branch; the barrier ends the peer reads of the tag gather first
+    int rc = dist_agree(a, who, {3.0});
+    if (rc || !empty) return rc;
+    set_error(std::string(who) + ": the new mesh has fewer blocks than ranks (" + std::to_string(nnew) + " for " +
+              std::to_string(W) + ")");
+    return CUP2D_EINVAL;
+  }
+  cup2d_amr *n = nullptr;
+  int rc = cup2d_amr_create_ranks(nnew, new_level_ij, bpdx, bpdy, a->h0, a->nu, me, W, rb.data(), a->device, &n);
+  if (rc) return rc;
+  auto fail = [&](int code) {
+    cup2d_amr_destroy(n);
+    return code;
+  };
+  // this rank's share: new blocks in [b0, b1), numbered locally; sources stay global
+  const int64_t b0 = rb[me], b1 = rb[me + 1];
+  auto mine = [&](int64_t g) { return g >= b0 && g < b1; };
+  std::vector<int2> pairs;
+  std::vector<int4> kids;
+  std::vector<int32_t> cdst, parents, child;
+  for (const int2 &p : C.pairs)
+    if (mine(p.x)) pairs.push_back(make_int2((int)(p.x - b0), p.y));
+  for (size_t g = 0; g < C.kids.size(); g++)
+    if (mine(C.cdst[g])) kids.push_back(C.kids[g]), cdst.push_back((int32_t)(C.cdst[g] - b0));
+  for (size_t q = 0; q < C.parents.size(); q++) {
+    bool any = false;
+    for (int c = 0; c < 4; c++) any |= mine(C.child_dst[4 * q + c]);
+    if (!any) continue;
+    parents.push_back(C.parents[q]);
+    for (int c = 0; c < 4; c++) child.push_back(mine(C.child_dst[4 * q + c]) ? (int32_t)(C.child_dst[4 * q + c] - b0) : -1);
+  }
+  std::vector<int64_t> rp[2];
+  std::vector<int32_t> sb[2], sc[2];
+  std::vector<double> w[2];
+  for (int k = 0; k < 2; k++)
+    if ((rc = amr_plan_subset_rows(a->plan, 4 + k, (int64_t)parents.size(), parents.data(), rp[k], sb[k], sc[k], w[k]))) return fail(rc);
+  const int fields[RG_NF] = {CUP2D_TMP, CUP2D_CHI, CUP2D_VEL, CUP2D_VOLD, CUP2D_PRES, CUP2D_POLD};
+  RgFields F;
+  RgPeer P;
+  memset(&P, 0, sizeof P);
+  F.off2[0] = 0;
+  for (int f = 0; f < RG_NF; f++) {
+    F.src[f] = nullptr, F.dst[f] = n->f[fields[f]], F.dim[f] = dim_of(fields[f]);
+    F.off2[f + 1] = F.off2[f] + 32 * F.dim[f];
+    for (int r = 0; r < W; r++) {
+      P.base[f][r] = static_cast<const double *>(cup2d_peer_field_ptr(a->poisson, r, fields[f]));
+      if (!P.base[f][r]) {
+        set_error(std::string(who) + ": peers not attached");
+        return fail(CUP2D_ESTATE);
+      }
+    }
+  }
+  for (int r = 0; r <= W; r++) P.rb[r] = orb[r];
+  P.nranks = W;
+  const int64_t np = (int64_t)pairs.size(), ng = (int64_t)kids.size(), nq = (int64_t)parents.size();
+  bool launched;
+  {
+    RgScratch S;
+    RgLab L = {};
+    for (int k = 0; k < 2; k++) L.rowptr[k] = S.up(rp[k]), L.sb[k] = S.up(sb[k]), L.sc[k] = S.up(sc[k]), L.w[k] = S.up(w[k]);
+    L.rbeg[0] = 0;
+    for (int f = 0; f < RG_NF; f++) L.rbeg[f + 1] = L.rbeg[f] + (int64_t)rp[F.dim[f] == 2 ? 0 : 1].size() - 1;
+    for (int f = 0; f < RG_NF; f++) L.lab[f] = S.get<double>((size_t)nq * 100 * F.dim[f]);
+    const int2 *d_pairs = S.up(pairs);
+    const int4 *d_kids = S.up(kids);
+    const int *d_cdst = S.up(cdst), *d_child = S.up(child);
+    if (!S.ok) {
+      set_error(std::string(who) + ": out of device memory");
+      return fail(CUP2D_ECUDA);
+    }
+    if (np) amr_regrid_peer_copy_kernel<<<rg_grid(np * F.off2[RG_NF]), 256, 0, a->stream>>>(F, P, d_pairs, np);
+    if (ng) amr_regrid_peer_compress_kernel<<<rg_grid(ng * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, P, d_cdst, d_kids, ng);
+    if (nq) {
+      amr_regrid_peer_lab_kernel<<<rg_grid(L.rbeg[RG_NF]), 256, 0, a->stream>>>(F, P, L);
+      amr_regrid_peer_refine_kernel<<<rg_grid(nq * 2 * F.off2[RG_NF]), 256, 0, a->stream>>>(F, L, d_child, nq);
+    }
+    launched = cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(a->stream) == cudaSuccess;
+  }
+  if (!launched) {
+    set_error(std::string(who) + ": transfer kernels failed");
+    return fail(CUP2D_ECUDA);
+  }
+  // every rank done reading before anyone frees its old arrays
+  if ((rc = dist_agree(a, who, {4.0}))) return fail(rc);
+  // one rank attaches itself; several re-exchange their blobs (cup2d_amr_peer_export / _attach) before the next peer call
+  const char none = 0;
+  if (W == 1 && (rc = cup2d_amr_peer_attach(n, &none))) return fail(rc);
+  const bool use_graph = a->use_graph;
+  std::swap(*a, *n); // a distributed context's stream belongs to its Poisson context: the new mesh's stream comes along
+  a->use_graph = use_graph;
+  cup2d_amr_destroy(n);
+  return CUP2D_OK;
+}
+
+// the distributed adapt / regrid entry: the argument check and barrier, then (adapt) the tags of every rank into d_linf
+// [nglobal]; `own` = this rank's tags on the device
+static int dist_gather_tags(cup2d_amr *a, const double *own, double *d_linf) {
+  const int W = a->nranks;
+  cup2d_sim *ps = a->poisson;
+  if (W > 1) { // this rank's tags into its Krylov scratch kz (exported, idle outside the Poisson solve), then a barrier
+    CUP2D_CUDA(cudaMemcpyAsync(ps->kz, own, (size_t)a->nb * sizeof(double), cudaMemcpyDeviceToDevice, a->stream));
+    int rc = dist_agree(a, "cup2d_amr_adapt", {2.0});
+    if (rc) return rc;
+  }
+  for (int r = 0; r < W; r++) {
+    const double *src = r == a->rank ? own : static_cast<const double *>(ps->peer_base[r][CUP2D_NFIELDS]);
+    CUP2D_CUDA(cudaMemcpyAsync(d_linf + a->rank_begin[r], src, (size_t)(a->rank_begin[r + 1] - a->rank_begin[r]) * sizeof(double),
+                               cudaMemcpyDeviceToDevice, a->stream));
+  }
+  return CUP2D_OK;
+}
+
 } // namespace cup2d
 
 using namespace cup2d;
@@ -482,20 +759,29 @@ extern "C" {
 
 /* Regrid in place onto new_level_ij[nblocks_new][3] (any order; cup2d_amr_adapt_mesh gives the reference's): see the head of
  * this file.  CUP2D_EINVAL (context untouched) if the new mesh is not one refine / compress step from the current one or not
- * 2:1 balanced; CUP2D_ESTATE for multi-rank contexts.  An identical block list is a no-op. */
+ * 2:1 balanced; CUP2D_ESTATE for contexts of cup2d_amr_set_ranks.  An identical block list is a no-op.  Distributed contexts:
+ * every rank passes the whole new list (regrid_apply_dist). */
 int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level_ij) {
   if (!a || nblocks_new <= 0 || !new_level_ij) {
     set_error("cup2d_amr_regrid: bad arguments");
     return CUP2D_EINVAL;
   }
-  if (a->dist || a->nranks > 1) {
-    set_error("cup2d_amr_regrid: contexts on several ranks cannot be regridded (blocks would have to migrate between ranks)");
+  if (a->nranks > 1 && !a->dist) {
+    set_error("cup2d_amr_regrid: contexts of cup2d_amr_set_ranks (operators replicated on several ranks) cannot be regridded");
     return CUP2D_ESTATE;
   }
   int bpdx = 0, bpdy = 0;
   const std::vector<int> &old = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
-  const int64_t nold = a->nb;
-  if (nblocks_new == nold && std::equal(old.begin(), old.end(), new_level_ij)) return CUP2D_OK;
+  const int64_t nold = a->dist ? a->nglobal : a->nb; // a distributed context's plan holds the whole list
+  if (a->dist) {
+    std::vector<double> args = {1.0, (double)nblocks_new};
+    list_hash(new_level_ij, nblocks_new, args);
+    CUP2D_CUDA(cudaSetDevice(a->device));
+    const int rc = dist_agree(a, "cup2d_amr_regrid", args);
+    if (rc) return rc;
+  } else if (nblocks_new == nold && std::equal(old.begin(), old.end(), new_level_ij)) {
+    return CUP2D_OK;
+  }
   std::map<std::array<int, 3>, int> index;
   for (int64_t k = 0; k < nold; k++) index[{old[3 * k], old[3 * k + 1], old[3 * k + 2]}] = (int)k;
   auto find = [&](int l, int i, int j) {
@@ -549,6 +835,11 @@ int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level
   }
   for (int64_t k = 0; k < nold; k++)
     if (used[k] != 1) return reject("old block " + std::to_string(k) + (used[k] ? " is used twice" : " is not covered"));
+  if (a->dist) {
+    bool changed = false;
+    return regrid_apply_dist(a, "cup2d_amr_regrid", nblocks_new, new_level_ij, bpdx, bpdy, RgPlanHost{pairs, kids, cdst, parents, child_dst},
+                             &changed);
+  }
   RgScratch S;
   const int2 *d_pairs = S.up(pairs);
   const int4 *d_kids = S.up(kids);
@@ -570,13 +861,13 @@ int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double 
     set_error("cup2d_amr_adapt: bad arguments");
     return CUP2D_EINVAL;
   }
-  if (a->dist || a->nranks > 1) {
-    set_error("cup2d_amr_adapt: contexts on several ranks cannot be regridded (blocks would have to migrate between ranks)");
+  if (a->nranks > 1 && !a->dist) {
+    set_error("cup2d_amr_adapt: contexts of cup2d_amr_set_ranks (operators replicated on several ranks) cannot be regridded");
     return CUP2D_ESTATE;
   }
   int bpdx = 0, bpdy = 0;
   const std::vector<int> &old = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
-  const int64_t nold = a->nb;
+  const int64_t nold = a->dist ? a->nglobal : a->nb; // a distributed context's plan holds the whole list
   if (((int64_t)std::max(bpdx, bpdy) << (level_max - 1)) >= (1 << 29)) {
     set_error("cup2d_amr_adapt: the finest level has 2^29 blocks or more per direction");
     return CUP2D_EINVAL;
@@ -587,13 +878,27 @@ int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double 
       return CUP2D_EINVAL;
     }
   CUP2D_CUDA(cudaSetDevice(a->device));
+  if (a->dist) {
+    const int rc = dist_agree(a, "cup2d_amr_adapt", {0.0, rtol, ctol, (double)level_max, block_linf ? 1.0 : 0.0});
+    if (rc) return rc;
+  }
   RgScratch S;
   const double *d_linf = a->d_part;
   if (block_linf) {
-    d_linf = S.up(std::vector<double>(block_linf, block_linf + nold));
+    d_linf = S.up(std::vector<double>(block_linf, block_linf + a->nb)); // a distributed context: this rank's blocks
   } else {
     const int rc = amr_adapt_tags_enqueue(a, rtol, level_max);
     if (rc) return rc;
+  }
+  if (a->dist) { // every rank's tags, in global block order
+    double *all = S.get<double>(nold);
+    if (!S.ok) {
+      set_error("cup2d_amr_adapt: out of device memory");
+      return CUP2D_ECUDA;
+    }
+    const int rc = dist_gather_tags(a, d_linf, all);
+    if (rc) return rc;
+    d_linf = all;
   }
   const int64_t npad = pow2_at_least(nold);
   const CurveTables tables(bpdx, bpdy);
@@ -654,6 +959,21 @@ int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double 
   CUP2D_CUDA(cudaMemcpyAsync(nl.data(), new_lij, nl.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
   if (nq) CUP2D_CUDA(cudaMemcpyAsync(parents.data(), d_parents, parents.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
   CUP2D_CUDA(cudaStreamSynchronize(stream));
+  if (a->dist) { // the global classification to the host: every rank takes its share of it
+    RgPlanHost C;
+    C.pairs.resize(np), C.kids.resize(ng), C.cdst.resize(ng), C.child_dst.resize(4 * nq);
+    C.parents = parents;
+    if (np) CUP2D_CUDA(cudaMemcpy(C.pairs.data(), d_pairs, np * sizeof(int2), cudaMemcpyDeviceToHost));
+    if (ng) CUP2D_CUDA(cudaMemcpy(C.kids.data(), d_kids, ng * sizeof(int4), cudaMemcpyDeviceToHost));
+    if (ng) CUP2D_CUDA(cudaMemcpy(C.cdst.data(), d_cdst, ng * sizeof(int), cudaMemcpyDeviceToHost));
+    if (nq) CUP2D_CUDA(cudaMemcpy(C.child_dst.data(), d_child, 4 * nq * sizeof(int), cudaMemcpyDeviceToHost));
+    bool changed = false;
+    const int rc = regrid_apply_dist(a, "cup2d_amr_adapt", nnew, nl.data(), bpdx, bpdy, C, &changed);
+    if (rc) return rc;
+    if (nblocks_out) *nblocks_out = nnew;
+    if (changed_out) *changed_out = changed;
+    return CUP2D_OK;
+  }
   const bool same = nnew == nold && std::equal(old.begin(), old.end(), nl.begin());
   const int rc = same ? CUP2D_OK : regrid_apply(a, "cup2d_amr_adapt", nnew, nl.data(), bpdx, bpdy, parents, d_pairs, np, d_kids,
                                                 d_cdst, ng, d_child);
@@ -661,6 +981,18 @@ int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double 
   if (nblocks_out) *nblocks_out = nnew;
   if (changed_out) *changed_out = !same;
   return CUP2D_OK;
+}
+
+/* the partition of the context's block list: rank_begin[nranks+1] (NULL: only nranks); {0, nb} for a plain context */
+int32_t cup2d_amr_rank_begin(const cup2d_amr *a, int64_t *rank_begin_out) {
+  if (!a) {
+    set_error("cup2d_amr_rank_begin: bad arguments");
+    return CUP2D_EINVAL;
+  }
+  const std::vector<int64_t> plain = {0, a->nb};
+  const std::vector<int64_t> &rb = a->rank_begin.empty() ? plain : a->rank_begin;
+  if (rank_begin_out) std::copy(rb.begin(), rb.end(), rank_begin_out);
+  return (int32_t)rb.size() - 1;
 }
 
 /* the context's block list [n][3] (level, i, j) into level_ij_out (NULL: only the count) */

@@ -34,7 +34,7 @@ SYMBOLS = [
     "cup2d_amr_ongrid_timing", "cup2d_amr_ongrid_times", "cup2d_amr_shape_set_dist", "cup2d_amr_collide",
     "cup2d_amr_surface", "cup2d_amr_surface_get", "cup2d_amr_forces", "cup2d_amr_udef_blend",
     "cup2d_amr_step_enqueue", "cup2d_amr_pressure_enqueue", "cup2d_amr_step_result", "cup2d_amr_set_graph",
-    "cup2d_amr_adapt", "cup2d_amr_blocks",
+    "cup2d_amr_adapt", "cup2d_amr_blocks", "cup2d_amr_rank_begin",
 ]
 
 
@@ -176,6 +176,7 @@ def load_library():
     lib.cup2d_amr_adapt.argtypes = [P, C.POINTER(D), D, D, I, C.POINTER(L), C.POINTER(C.c_int32)]
     lib.cup2d_amr_blocks.argtypes = [P, C.POINTER(C.c_int32)]
     lib.cup2d_amr_blocks.restype = L
+    lib.cup2d_amr_rank_begin.argtypes = [P, C.POINTER(C.c_int64)]
     lib.cup2d_amr_ongrid.argtypes = [P, I, C.POINTER(Body), C.POINTER(D)]
     lib.cup2d_amr_ongrid_timing.argtypes = [P, I]
     lib.cup2d_amr_ongrid_times.argtypes = [P, C.POINTER(D)]

@@ -368,7 +368,9 @@ int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t b
  * (main.cpp:5012-5028), compresses by the reference's 4-cell average (5160-5164) for tmp, chi, vel, vold, pres, pold; tmpV is
  * zero afterwards.  Plan, tables, Poisson context and lab buffers are rebuilt for the new mesh; shapes are cleared (set them
  * again, as ongrid() does after adapt()).  CUP2D_EINVAL, context untouched, for a mesh that is not one step away;
- * CUP2D_ESTATE for contexts on several ranks.  The same block list is a no-op. */
+ * CUP2D_ESTATE for contexts of cup2d_amr_set_ranks.  The same block list is a no-op.
+ * On a distributed context (cup2d_amr_create_ranks, one rank included) every rank makes the call with the whole new list:
+ * the ranks move onto the reference's new partition (see cup2d_amr_adapt) and read old blocks over the peer mapping. */
 int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level_ij);
 /* adapt() in one call, decision included (csrc/amr_regrid.cu): block_linf == NULL runs cup2d_amr_adapt_tags on the device
  * without downloading it (the tagging field is left in tmp as there); otherwise block_linf[nblocks] are the caller's per-block
@@ -377,9 +379,23 @@ int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level
  * the same fields.  Only the new block list and the refined parents cross to the host.  An unchanged list is a no-op after
  * the tagging.  nblocks_out (new block count) and changed_out (0 / 1) may be NULL; cup2d_amr_blocks reads the new list.
  * CUP2D_EINVAL, context untouched, for level_max outside 1..20 or a block at or above level_max; CUP2D_ESTATE for contexts
- * on several ranks. */
+ * of cup2d_amr_set_ranks.
+ * On a distributed context (cup2d_amr_create_ranks, one rank included) every rank makes the call with the same arguments;
+ * block_linf, if not NULL, holds this rank's own blocks.  Tags, decision and new list are global (the same on every rank);
+ * the new partition is the reference's load balancing (main.cpp:5196-5205, 5332-5349): with n_r the new blocks rank r
+ * produces (a copy or a child on the old block's rank, a compressed parent on the rank of its even-i, even-j sibling), every
+ * rank gets total / nranks (the first total % nranks one more) if max n / min n > 1.01 or min n == 0, otherwise
+ * (n_r - n_{r+1}) / 4 (truncated) blocks move from rank r to r+1.  changed_out is 1 if the list or the partition changed;
+ * cup2d_amr_rank_begin reads the new partition.  With several ranks a change puts the fields in new arrays: every rank
+ * calls cup2d_amr_peer_export / _attach again, and until then calls that reach a peer return CUP2D_ESTATE (one rank
+ * attaches itself).  CUP2D_ECOMM on every rank, contexts kept, if the ranks pass different arguments; CUP2D_EINVAL on
+ * every rank, contexts kept, if the new mesh has fewer blocks than ranks.  Bitwise the fields of the plain context's call,
+ * rank by rank. */
 int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double ctol, int level_max, int64_t *nblocks_out,
                     int32_t *changed_out);
+/* the partition of the context's block list: returns nranks and writes rank_begin[nranks+1] (NULL: only nranks); a plain
+ * context returns 1 with {0, nb} */
+int32_t cup2d_amr_rank_begin(const cup2d_amr *a, int64_t *rank_begin_out);
 /* the context's block list, [n][3] (level, i, j), into level_ij_out; NULL: only the count n */
 int64_t cup2d_amr_blocks(const cup2d_amr *a, int32_t *level_ij_out);
 
