@@ -236,7 +236,9 @@ class AmrSimulation:
 
     def step_enqueue(self, cfl=0.5, dt=0.0, tol_abs=0.0, tol_rel=0.0, max_restarts=0, max_iter=1000):
         """step() without host synchronisation (cup2d_amr_step_enqueue): dt <= 0 runs the dt rule on the device; read the
-        outcome with step_result()"""
+        outcome with step_result().  On a distributed context every rank makes the same calls with the same arguments; dt's
+        maximum and the pressure means are all-reduced on the device, so every rank gets the same (dt, iterations,
+        residual)"""
         _l.check(self.lib.cup2d_amr_step_enqueue(self._h, float(cfl), float(dt), float(tol_abs), float(tol_rel), int(max_restarts),
                                                  int(max_iter)))
 
@@ -252,7 +254,8 @@ class AmrSimulation:
         return dto.value, it.value, err.value
 
     def set_graph(self, on=True):
-        """on: from the second enqueue of a form, replay it as one CUDA graph (default); off: launch the kernels directly"""
+        """on: from the second enqueue of a form, replay it as one CUDA graph (default); off: launch the kernels directly.
+        Plain and distributed contexts; a context of set_ranks has the blocking calls only"""
         _l.check(self.lib.cup2d_amr_set_graph(self._h, int(on)))
 
     def set_ranks(self, rank, rank_begin, dist=None):

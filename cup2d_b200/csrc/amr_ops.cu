@@ -347,6 +347,17 @@ static int fluxcorr(cup2d_amr *a, const double *labA, const double *labB, double
 
 using namespace cup2d;
 
+#ifndef CUP2D_AMR_EMU
+// the executable graphs of enqueued steps (an in-flight launch completes before its graph is freed)
+static void amr_drop_graphs(cup2d_amr *a) {
+  for (auto &g : a->graphs) {
+    if (g.exec) cudaGraphExecDestroy((cudaGraphExec_t)g.exec);
+    if (g.graph) cudaGraphDestroy((cudaGraph_t)g.graph);
+  }
+  a->graphs.clear();
+}
+#endif
+
 #define CHECK_AMR(a)                                                                              \
   if (!(a)) {                                                                                     \
     cup2d::set_error("null cup2d_amr handle");                                                    \
@@ -444,10 +455,7 @@ void cup2d_amr_destroy(cup2d_amr *a) {
     cudaFree(g.grow); cudaFree(g.rowptr); cudaFree(g.dst); cudaFree(g.sb); cudaFree(g.sc); cudaFree(g.w);
   }
 #ifndef CUP2D_AMR_EMU
-  for (auto &g : a->graphs) {
-    if (g.exec) cudaGraphExecDestroy((cudaGraphExec_t)g.exec);
-    if (g.graph) cudaGraphDestroy((cudaGraph_t)g.graph);
-  }
+  amr_drop_graphs(a);
   if (a->ev_fork) cudaEventDestroy((cudaEvent_t)a->ev_fork);
   if (a->ev_join) cudaEventDestroy((cudaEvent_t)a->ev_join);
   if (a->poisson) cup2d_destroy(a->poisson);
@@ -933,6 +941,7 @@ int cup2d_amr_peer_attach(cup2d_amr *a, const void *all_blobs) {
     set_error("cup2d_amr_peer_attach: call cup2d_amr_set_ranks first");
     return CUP2D_ESTATE;
   }
+  amr_drop_graphs(a); // their halo pulls and all-reduces hold the peer pointers of the previous attach
   return cup2d_peer_attach(a->poisson, all_blobs);
 }
 
@@ -1023,7 +1032,9 @@ int cup2d_amr_step(cup2d_amr *a, double cfl, double dt_in, double tol_abs, doubl
 // the Krylov solve.  Here dt lives in the device record a->d_rec and every dt-dependent kernel reads it from there
 // (OnDevice), the means are reduced on the device into the same record, and the solve is enqueued on the Poisson context's
 // stream, joined to this one by events: nothing in the body depends on a host value that changes from step to step, so it
-// is captured once per argument set into a CUDA graph and replayed with one cudaGraphLaunch.
+// is captured once per argument set into a CUDA graph and replayed with one cudaGraphLaunch.  A distributed context
+// (cup2d_amr_create_ranks) runs the same body on its Poisson context's stream and arrays: the solve in place, the halo
+// refreshes as stream-ordered peer pulls, dt's maximum and the means all-reduced by warp 0 of the one-CTA reductions.
 namespace cup2d {
 
 constexpr int AMR_RED_NT = 1024; // one CTA reduces the per-block partials of the whole mesh
@@ -1031,10 +1042,11 @@ constexpr int AMR_RED_NT = 1024; // one CTA reduces the per-block partials of th
 // dt given by value: written by a kernel ahead of the graph launch, so that the graph does not hold it
 __global__ void amr_set_dt_kernel(double *rec, double dt) { rec[AMR_REC_DT] = dt; }
 
-// the dt rule of cup2d_amr_compute_dt: the largest per-block maximum (a maximum is exact in any order), then main.cpp:6593-6595
-// in the host code's operation order with explicit round-to-nearest operations (no FMA contraction): bitwise the host's dt
+// the dt rule of cup2d_amr_compute_dt: the largest per-block maximum (a maximum is exact in any order), on a distributed
+// context all-reduced over the ranks by warp 0 (peer_allreduce returns at once on one rank), then main.cpp:6593-6595 in the
+// host code's operation order with explicit round-to-nearest operations (no FMA contraction): bitwise the host's dt
 __global__ void __launch_bounds__(AMR_RED_NT) amr_dt_kernel(const double *__restrict__ part, int64_t nb, double h, double nu,
-                                                            double cfl, double *rec) {
+                                                            double cfl, double *rec, Comm comm) {
   __shared__ double sm[AMR_RED_NT];
   double m = 0.0;
   for (int64_t k = threadIdx.x; k < nb; k += AMR_RED_NT) m = fmax(m, part[k]);
@@ -1044,8 +1056,10 @@ __global__ void __launch_bounds__(AMR_RED_NT) amr_dt_kernel(const double *__rest
     if ((int)threadIdx.x < s) sm[threadIdx.x] = fmax(sm[threadIdx.x], sm[threadIdx.x + s]);
     __syncthreads();
   }
+  if (threadIdx.x >= 32) return;
+  double umax = sm[0], none[1] = {0.0};
+  peer_allreduce<1>(comm, none, umax, threadIdx.x);
   if (threadIdx.x == 0) {
-    const double umax = sm[0];
     const double dt_diff = __ddiv_rn(__dmul_rn(__dmul_rn(0.25, h), h), __dadd_rn(nu, __dmul_rn(__dmul_rn(0.25, h), umax)));
     const double dt_adv = __ddiv_rn(h, __dadd_rn(umax, 1e-8));
     const double c = __dmul_rn(cfl, dt_adv);
@@ -1055,9 +1069,11 @@ __global__ void __launch_bounds__(AMR_RED_NT) amr_dt_kernel(const double *__rest
 
 // sum(P h^2) / sum(h^2) over the per-block pairs of amr_block_wsum_kernel in a FIXED order, so that a step gives the same bits
 // every time: thread t adds the blocks t, t + NT, t + 2 NT, ... in block order, then the NT partial sums are combined by a
-// binary tree (s[t] += s[t + m] for m = NT/2, ..., 1).  The blocking path adds the blocks in one serial chain on the host;
-// the two orders agree to rounding.
-__global__ void __launch_bounds__(AMR_RED_NT) amr_wmean_kernel(const double *__restrict__ part, int64_t nb, double *mean) {
+// binary tree (s[t] += s[t + m] for m = NT/2, ..., 1).  On a distributed context warp 0 then all-reduces the rank's pair
+// (sum P h^2, sum h^2), the ranks' pairs added in rank order, so every rank divides the same bits (one rank: no-op).  The
+// blocking path adds the blocks in one serial chain on the host; the two orders agree to rounding.
+__global__ void __launch_bounds__(AMR_RED_NT) amr_wmean_kernel(const double *__restrict__ part, int64_t nb, double *mean,
+                                                               Comm comm) {
   __shared__ double ss[AMR_RED_NT];
   __shared__ double sw[AMR_RED_NT];
   const double2 *p2 = reinterpret_cast<const double2 *>(part);
@@ -1079,7 +1095,10 @@ __global__ void __launch_bounds__(AMR_RED_NT) amr_wmean_kernel(const double *__r
     if ((int)threadIdx.x < m) ss[threadIdx.x] += ss[threadIdx.x + m], sw[threadIdx.x] += sw[threadIdx.x + m];
     __syncthreads();
   }
-  if (threadIdx.x == 0) *mean = ss[0] / sw[0];
+  if (threadIdx.x >= 32) return;
+  double sum[2] = {ss[0], sw[0]}, none = 0.0;
+  peer_allreduce<2>(comm, sum, none, threadIdx.x);
+  if (threadIdx.x == 0) *mean = sum[0] / sum[1];
 }
 
 // dst = the Krylov iterate the solve returns (KrylovState::opt, chosen on the device)
@@ -1098,7 +1117,7 @@ static int pressure_correct_enqueued(cup2d_amr *a) {
   for (int pass = 0; pass < 2; pass++) { // pres -= mean_h2(pres); then pres += pold - mean_h2(pres)
     double *mean = a->d_rec + AMR_REC_MEAN0 + pass;
     amr_block_wsum_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->f[CUP2D_PRES], a->d_h, a->d_part, a->nb);
-    amr_wmean_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, mean);
+    amr_wmean_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, mean, a->poisson->comm);
     amr_shift_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], nullptr, pass ? a->f[CUP2D_POLD] : nullptr, n,
                                                          OnDevice{mean});
     CUP2D_CUDA(cudaGetLastError());
@@ -1119,16 +1138,23 @@ static int enqueue_body(cup2d_amr *a, bool pressure_only, bool dev_dt, double cf
   if (!pressure_only) {
     if (dev_dt) {
       amr_block_absmax_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->f[CUP2D_VEL], a->d_part, a->nb);
-      amr_dt_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, a->hmin, a->nu, cfl, a->d_rec);
+      amr_dt_kernel<<<1, AMR_RED_NT, 0, a->stream>>>(a->d_part, a->nb, a->hmin, a->nu, cfl, a->d_rec, a->poisson->comm);
       CUP2D_CUDA(cudaGetLastError());
     }
     if ((rc = rk2(a, 0.0, ddt))) return rc;
     CUP2D_CUDA(cudaMemsetAsync(a->f[CUP2D_TMPV], 0, (size_t)n * 2 * sizeof(double), a->stream)); // no bodies: u_def = 0
   }
   if ((rc = poisson_rhs(a, 0.0, ddt))) return rc;
+  cup2d_sim *ps = a->poisson;
+  if (a->dist) { // stream and fields are the Poisson context's: b = tmp and x0 = pres in place, as the blocking solve
+    if ((rc = poisson_enqueue(ps, tol_abs, tol_rel, max_restarts, max_iter, capturing))) return rc;
+    // this rank's blocks; the pressure gradient refreshes the halo slots of pres itself
+    amr_take_x_kernel<<<grid_for(n), 256, 0, a->stream>>>(a->f[CUP2D_PRES], ps->kx[0], ps->kx[1], ps->kx[2], ps->d_state, n);
+    CUP2D_CUDA(cudaGetLastError());
+    return pressure_correct_enqueued(a);
+  }
   // b = tmp, x0 = pres into the Poisson context, on its stream after this one's work (the event also pulls that stream
   // into a capture of this one); the iterate comes back after the solve's last kernel
-  cup2d_sim *ps = a->poisson;
   CUP2D_CUDA(cudaEventRecord((cudaEvent_t)a->ev_fork, a->stream));
   CUP2D_CUDA(cudaStreamWaitEvent(ps->stream, (cudaEvent_t)a->ev_fork, 0));
   CUP2D_CUDA(cudaMemcpyAsync(ps->f[CUP2D_TMP], a->f[CUP2D_TMP], n * sizeof(double), cudaMemcpyDeviceToDevice, ps->stream));
@@ -1144,8 +1170,14 @@ static int enqueue_body(cup2d_amr *a, bool pressure_only, bool dev_dt, double cf
 static int amr_enqueue(cup2d_amr *a, const char *who, bool pressure_only, double cfl, double dt_in, double tol_abs,
                        double tol_rel, int max_restarts, int max_iter) {
   CHECK_AMR(a);
-  if (a->dist || !a->rank_begin.empty()) {
-    set_error(std::string(who) + ": contexts on several ranks have the blocking calls only");
+  if (!a->dist && !a->rank_begin.empty()) {
+    set_error(std::string(who) + ": contexts of cup2d_amr_set_ranks have the blocking calls only");
+    return CUP2D_ESTATE;
+  }
+  // a distributed context's kernels pull halos and all-reduce through the peer mapping, and a graph keeps its pointers:
+  // nothing before the attach (a fresh context, or one whose regrid moved it onto new arrays)
+  if (a->dist && a->nranks > 1 && !a->poisson->peers_attached) {
+    set_error(std::string(who) + ": distributed context before cup2d_amr_peer_attach");
     return CUP2D_ESTATE;
   }
   const bool dev_dt = !(dt_in > 0);
@@ -1158,7 +1190,7 @@ static int amr_enqueue(cup2d_amr *a, const char *who, bool pressure_only, double
   int rc;
   if ((rc = ensure_poisson(a))) return rc;
   if (!a->d_rec) CUP2D_CUDA(cudaMalloc(&a->d_rec, AMR_REC_N * sizeof(double)));
-  if (!a->ev_fork) {
+  if (!a->dist && !a->ev_fork) {
     cudaEvent_t f, j;
     CUP2D_CUDA(cudaEventCreateWithFlags(&f, cudaEventDisableTiming));
     a->ev_fork = f;
@@ -1252,8 +1284,8 @@ int cup2d_amr_step_result(cup2d_amr *a, double *dt_out, int *iters_out, double *
 
 int cup2d_amr_set_graph(cup2d_amr *a, int on) {
   CHECK_AMR(a);
-  if (a->dist || !a->rank_begin.empty()) {
-    set_error("cup2d_amr_set_graph: contexts on several ranks have the blocking calls only");
+  if (!a->dist && !a->rank_begin.empty()) {
+    set_error("cup2d_amr_set_graph: contexts of cup2d_amr_set_ranks have the blocking calls only");
     return CUP2D_ESTATE;
   }
   a->use_graph = on != 0;

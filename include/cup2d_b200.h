@@ -312,12 +312,18 @@ int cup2d_amr_poisson_solve(cup2d_amr *a, double tol_abs, double tol_rel, int ma
 int cup2d_amr_pressure_correct(cup2d_amr *a, double dt);
 int cup2d_amr_step(cup2d_amr *a, double cfl, double dt_in, double tol_abs, double tol_rel, int max_restarts, int max_iter,
                    double *dt_out, int *iters, double *err);
-/* Enqueued forms, without host synchronisation (one GPU, single-rank contexts only: contexts of cup2d_amr_set_ranks or
- * cup2d_amr_create_ranks return CUP2D_ESTATE).  dt, the two pressure means and the Krylov stopping rule stay on the device;
- * from the second enqueue of a form on a mesh, each enqueue is one CUDA graph launch (one graph per argument set, rebuilt
- * after cup2d_amr_regrid).  Several enqueues may come before one result.  Bad arguments return CUP2D_EINVAL with the
- * context untouched.  dt equals cup2d_amr_compute_dt's bit for bit; the means are summed in a fixed order on the device
- * (DESIGN.md 7.1), so fields agree with the blocking calls to rounding.
+/* Enqueued forms, without host synchronisation, on plain contexts and on distributed contexts (cup2d_amr_create_ranks, one
+ * rank included); contexts of cup2d_amr_set_ranks return CUP2D_ESTATE.  dt, the two pressure means and the Krylov stopping
+ * rule stay on the device; from the second enqueue of a form on a mesh, each enqueue is one CUDA graph launch (one graph per
+ * argument set, rebuilt after cup2d_amr_regrid / cup2d_amr_adapt and after cup2d_amr_peer_attach).  Several enqueues may
+ * come before one result.  Bad arguments return CUP2D_EINVAL with the context untouched.  dt equals cup2d_amr_compute_dt's
+ * bit for bit; the means are summed in a fixed order on the device (DESIGN.md 7.1), so fields agree with the blocking calls
+ * to rounding.
+ * Distributed contexts: every rank makes the same calls with the same arguments, as with the blocking form.  dt's maximum
+ * and the means' two sums are all-reduced over the ranks inside the reduction kernels, so dt, iterations and residual are
+ * the same bits on every rank; a one-rank distributed context steps bit for bit like a plain context.  With several ranks,
+ * CUP2D_ESTATE (nothing enqueued, fields untouched) until cup2d_amr_peer_attach has run, also after a regrid that moved the
+ * arrays; cup2d_amr_step_result returns CUP2D_ECOMM if a peer never arrived at a halo pull or an all-reduce.
  * cup2d_amr_step_enqueue: cup2d_amr_step (no bodies); dt_in <= 0 runs the dt rule of cup2d_amr_compute_dt with cfl on the
  * device. */
 int cup2d_amr_step_enqueue(cup2d_amr *a, double cfl, double dt_in, double tol_abs, double tol_rel, int max_restarts, int max_iter);
@@ -341,7 +347,8 @@ int cup2d_amr_set_ranks(cup2d_amr *a, int32_t rank, int32_t nranks, const int64_
  * remote block its tables name, and computes only its own blocks.  Its field arrays are those of the distributed Poisson
  * context, so halo refreshes are the whole-block peer pulls of the uniform path, the solve runs in place, the face fluxes of
  * fillcases cross a rank boundary inside a field array, and dt / the pressure means are all-reduced in a kernel.  Fast kernels
- * only; cup2d_amr_field_upload / _download move this rank's blocks.  Follow with cup2d_amr_peer_export / _attach. */
+ * only; cup2d_amr_field_upload / _download move this rank's blocks.  Follow with cup2d_amr_peer_export / _attach (an attach
+ * drops the context's step graphs: they hold the peer pointers of the previous one). */
 int cup2d_amr_create_ranks(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, double h0, double nu,
                            int32_t rank, int32_t nranks, const int64_t *rank_begin, int32_t device, cup2d_amr **out);
 int cup2d_amr_peer_export(cup2d_amr *a, void *blob);
