@@ -1,6 +1,7 @@
 // Shared declarations of the multi-level device path (csrc/amr_ops.cu: table-gather baseline; csrc/amr_fast.cu: per-block
 // lab loader on the WENO line core).  See amr_ops.cu for the status of this path.
 #pragma once
+#include <algorithm>
 #include <vector>
 
 struct cup2d_amr_plan;
@@ -73,6 +74,27 @@ template <class F> inline int with_scalar(double v, const double *p, F &&launch)
 // the record an enqueued step keeps on the device: its dt, the two h^2-weighted pressure means
 enum { AMR_REC_DT = 0, AMR_REC_MEAN0 = 1, AMR_REC_MEAN1 = 2, AMR_REC_N = 4 };
 
+// lab entries per block of the compact ghost kinds 0-3 and 6 (cup2d_amr_plan_ghosts: dst = irregular position * this + entry)
+constexpr int GHOST_NCELL[7] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10, 16 * 16, 0, 0, 16 * 16 * 2};
+
+// h into a new device buffer of at least one element
+template <class T> inline cudaError_t upload(T **d, const std::vector<T> &h) {
+  const cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
+  if (e != cudaSuccess) return e;
+  return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
+}
+
+// The plan's tables on the host (csrc/amr_fast.cu), blocks named by their position in the whole list
+struct PlanGhosts { // cup2d_amr_plan_ghosts of one kind
+  std::vector<int64_t> rowptr;
+  std::vector<int32_t> dst, sb, sc;
+  std::vector<double> w;
+};
+int plan_ghosts(cup2d_amr *a, int which, PlanGhosts &g);
+int plan_neighbours(cup2d_amr *a, std::vector<int32_t> &n8); // [nglobal][8], cup2d_amr_plan_neighbours
+std::vector<int32_t> plan_irregular(cup2d_amr *a);
+std::vector<int32_t> plan_faces(cup2d_amr *a);                // [faces][5], cup2d_amr_plan_faces
+
 } // namespace cup2d
 
 // the dt-dependent operators with dt by value (ddt = nullptr) or from the device record of an enqueued step (csrc/amr_fast.cu)
@@ -90,8 +112,13 @@ struct cup2d_amr;
 // adapt()'s tagging (cup2d_amr_adapt_tags) enqueued on the context's stream: the tagging field in tmp, the per-block L-inf in
 // d_part[0..nb) (csrc/amr_ops.cu)
 extern "C" int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max);
-// single-rank contexts: the fast path's neighbour / irregular-block / compact ghost tables (csrc/amr_fast.cu), built on first use
+// the fast path's neighbour / irregular-block / compact ghost tables of kinds 0-2 (csrc/amr_fast.cu): amr_fast_tables builds
+// them on first use on a single-rank context (a no-op on a distributed one), amr_fast_build builds them now
 int amr_fast_tables(cup2d_amr *a);
+int amr_fast_build(cup2d_amr *a);
+// the compact ghost rows of stencil kind `which` of the context's irregular blocks into gt[which], every source by its slot
+// (csrc/amr_fast.cu); CUP2D_EINVAL if a source is not a halo slot
+int amr_ghost_rows(cup2d_amr *a, int which);
 // the per-block (i, j) table on the device, built on first use (csrc/penalize.cu)
 int amr_ensure_ij(cup2d_amr *a);
 // distributed contexts (cup2d_amr_create_ranks): refresh the halo slots of `field` from the owners (whole-block peer pulls,
@@ -103,11 +130,6 @@ extern "C" int amr_dist_sum(cup2d_amr *a, double *v, int n);
 // ranks' values added in rank order, so every rank gets the same bits; CUP2D_ECOMM if the ranks pass different n or a peer
 // never arrives.  A no-op otherwise (one rank included).
 extern "C" int amr_dist_sum_vec(cup2d_amr *a, double *v, int n);
-// fast-kernel tables of a distributed context for its block range [b0, b1): slot_of[global block] = local slot or -1
-int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64_t b0, int64_t b1);
-// distributed contexts: the compact ghost rows of stencil kind `which` (ncell lab entries per block) of the context's own
-// irregular blocks, every source named by its local slot (csrc/amr_fast.cu); CUP2D_EINVAL if a source is not a halo slot
-int amr_ghosts_dist(cup2d_amr *a, int which, int ncell, cup2d::GhostDev &g);
 
 struct cup2d_amr {
   int64_t nb = 0;
@@ -130,14 +152,15 @@ struct cup2d_amr {
   int rank = 0, nranks = 1;
   std::vector<int64_t> rank_begin;
   bool dist = false;                // cup2d_amr_create_ranks: this context holds only its own block range (+ halo slots)
-  int64_t gbegin = 0, nglobal = 0;  // distributed contexts: first own block in the global list, size of that list
+  int64_t gbegin = 0, nglobal = 0;  // the context's blocks are [gbegin, gbegin + nb) of the plan's list of nglobal blocks
   std::vector<int32_t> slot_of;     // distributed contexts: global block -> local slot (own blocks, then halo slots) or -1
+  int32_t slot(int64_t g) const { return dist ? slot_of[g] : (int32_t)g; } // where block g of the list lives here, or -1
   // fast paths (csrc/amr_fast.cu)
   bool fast = false;                // cup2d_amr_set_fast: the operator entry points dispatch to the fast kernels
   int *d_nbr4 = nullptr;            // [nb][4] W,E,S,N: same-level block, -1 wall, -2 coarser/finer
   int *d_irr_of = nullptr;          // [nb] position in the irregular list or -1
   int64_t nirr = 0;
-  cup2d::GhostDev gt[7];            // compact ghost tables per stencil kind (cup2d_amr_plan_ghosts): 0-2 with the fast tables,
+  cup2d::GhostDev gt[7];            // compact ghost tables per stencil kind (amr_ghost_rows): 0-2 with the fast tables,
                                     // 3 and 6 (the force diagnostics' labs, csrc/amr_forces.cu) on first use
   int *d_nbr8 = nullptr;            // [nb][8] cup2d_amr_plan_neighbours on the device (csrc/amr_forces.cu, first use)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)

@@ -17,17 +17,9 @@
 // correction kernel below, which is the coarse-face formulation of fillcases (see amr_ops.cu) reading those buffers.
 #include "sim.h"
 #include "weno.cuh"
-#include <map>
 #include <algorithm>
 #include <vector>
 #include "amr.h"
-
-extern "C" {
-int64_t cup2d_amr_plan_irregular(cup2d_amr_plan *p, int32_t *blocks_out);
-int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int64_t *rowptr, int32_t *dst, int32_t *src_block,
-                              int32_t *src_cellcomp, double *weight);
-int cup2d_amr_plan_neighbours(cup2d_amr_plan *p, int32_t *out);
-}
 
 namespace cup2d {
 
@@ -323,54 +315,111 @@ static int fast_constants() {
   return CUP2D_OK;
 }
 
-static int fast_setup(cup2d_amr *a) {
-  if (a->d_faceflux || a->dist) return CUP2D_OK; // distributed contexts get their tables from amr_fast_setup_dist
-  const int64_t nb = a->nb;
-  std::vector<int32_t> n8(8 * nb), n4(4 * nb), irr_of(nb, -1);
-  if (cup2d_amr_plan_neighbours(a->plan, n8.data())) return CUP2D_EINVAL;
-  for (int64_t k = 0; k < nb; k++) { // order of the 8: (-1,-1),(0,-1),(1,-1),(-1,0),(1,0),(-1,1),(0,1),(1,1)
-    const int pick[4] = {3, 4, 1, 6};  // W, E, S, N
-    for (int j = 0; j < 4; j++) n4[4 * k + j] = n8[8 * k + pick[j]] < -1 ? -2 : n8[8 * k + pick[j]];
-  }
-  const int64_t nirr = cup2d_amr_plan_irregular(a->plan, nullptr);
-  std::vector<int32_t> irr(std::max<int64_t>(nirr, 1));
-  cup2d_amr_plan_irregular(a->plan, irr.data());
-  for (int64_t qi = 0; qi < nirr; qi++) irr_of[irr[qi]] = (int32_t)qi;
-  a->nirr = nirr;
-  auto up = [](auto **d, const auto &h) -> cudaError_t {
-    using T = typename std::remove_reference<decltype(h[0])>::type;
-    cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  };
-  const int ncell[3] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10};
-  for (int which = 0; which < 3; which++) {
-    int64_t nrows = 0;
-    const int64_t nnz = cup2d_amr_plan_ghosts(a->plan, which, &nrows, nullptr, nullptr, nullptr, nullptr, nullptr);
-    if (nnz < 0) return CUP2D_EINVAL;
-    std::vector<int64_t> rp(nrows + 1), grow(nirr + 1, nrows);
-    std::vector<int32_t> dst(std::max<int64_t>(nrows, 1)), sb(std::max<int64_t>(nnz, 1)), sc(std::max<int64_t>(nnz, 1));
-    std::vector<double> w(std::max<int64_t>(nnz, 1));
-    cup2d_amr_plan_ghosts(a->plan, which, &nrows, rp.data(), dst.data(), sb.data(), sc.data(), w.data());
-    for (int64_t row = nrows - 1; row >= 0; row--) grow[dst[row] / ncell[which]] = row; // rows are grouped by block, in order
-    for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]); // blocks without rows
-    GhostDev &g = a->gt[which];
-    CUP2D_CUDA(up(&g.grow, grow));
-    CUP2D_CUDA(up(&g.rowptr, rp));
-    CUP2D_CUDA(up(&g.dst, dst));
-    CUP2D_CUDA(up(&g.sb, sb));
-    CUP2D_CUDA(up(&g.sc, sc));
-    CUP2D_CUDA(up(&g.w, w));
-  }
-  CUP2D_CUDA(up(&a->d_nbr4, n4));
-  CUP2D_CUDA(up(&a->d_irr_of, irr_of));
-  CUP2D_CUDA(cudaMalloc(&a->d_faceflux, std::max<int64_t>(nirr, 1) * 64 * sizeof(double)));
-  return fast_constants();
+int plan_ghosts(cup2d_amr *a, int which, PlanGhosts &g) {
+  int64_t nrows = 0;
+  const int64_t nnz = cup2d_amr_plan_ghosts(a->plan, which, &nrows, nullptr, nullptr, nullptr, nullptr, nullptr);
+  if (nnz < 0) return CUP2D_EINVAL;
+  g.rowptr.resize(nrows + 1), g.dst.resize(nrows), g.sb.resize(nnz), g.sc.resize(nnz), g.w.resize(nnz);
+  cup2d_amr_plan_ghosts(a->plan, which, &nrows, g.rowptr.data(), g.dst.data(), g.sb.data(), g.sc.data(), g.w.data());
+  return CUP2D_OK;
 }
+int plan_neighbours(cup2d_amr *a, std::vector<int32_t> &n8) {
+  n8.resize(8 * a->nglobal);
+  return cup2d_amr_plan_neighbours(a->plan, n8.data()) ? CUP2D_EINVAL : CUP2D_OK;
+}
+std::vector<int32_t> plan_irregular(cup2d_amr *a) {
+  std::vector<int32_t> irr(cup2d_amr_plan_irregular(a->plan, nullptr));
+  cup2d_amr_plan_irregular(a->plan, irr.data());
+  return irr;
+}
+std::vector<int32_t> plan_faces(cup2d_amr *a) {
+  std::vector<int32_t> rec(5 * cup2d_amr_plan_faces(a->plan, nullptr));
+  cup2d_amr_plan_faces(a->plan, rec.data());
+  return rec;
+}
+
+// plain contexts build the tables on first use; distributed ones have them from cup2d_amr_create_ranks
+static int fast_setup(cup2d_amr *a) { return a->d_faceflux || a->dist ? CUP2D_OK : amr_fast_build(a); }
 
 } // namespace cup2d
 
 int amr_fast_tables(cup2d_amr *a) { return cup2d::fast_setup(a); }
+
+// The plan's rows of the irregular blocks in [gbegin, gbegin + nb), renumbered to the context's irregular list (local
+// position * ncell + lab entry), every source by its slot.
+int amr_ghost_rows(cup2d_amr *a, int which) {
+  using namespace cup2d;
+  const int64_t b0 = a->gbegin, b1 = a->gbegin + a->nb;
+  const int ncell = GHOST_NCELL[which];
+  const std::vector<int32_t> irr = plan_irregular(a);
+  std::vector<int32_t> local_of_irr(irr.size(), -1);
+  int64_t nirr = 0;
+  for (size_t qi = 0; qi < irr.size(); qi++)
+    if (irr[qi] >= b0 && irr[qi] < b1) local_of_irr[qi] = (int32_t)nirr++;
+  PlanGhosts all, g;
+  int rc = plan_ghosts(a, which, all);
+  if (rc) return rc;
+  g.rowptr.reserve(all.rowptr.size()), g.dst.reserve(all.dst.size());
+  g.sb.reserve(all.sb.size()), g.sc.reserve(all.sc.size()), g.w.reserve(all.w.size());
+  g.rowptr.push_back(0);
+  for (size_t row = 0; row < all.dst.size(); row++) {
+    const int32_t ql = local_of_irr[all.dst[row] / ncell];
+    if (ql < 0) continue;
+    g.dst.push_back(ql * ncell + all.dst[row] % ncell);
+    for (int64_t e = all.rowptr[row]; e < all.rowptr[row + 1]; e++) {
+      const int32_t sl = a->slot(all.sb[e]);
+      if (sl < 0) {
+        set_error("distributed context: a lab source lies outside the halo set");
+        return CUP2D_EINVAL;
+      }
+      g.sb.push_back(sl);
+      g.sc.push_back(all.sc[e]);
+      g.w.push_back(all.w[e]);
+    }
+    g.rowptr.push_back((int64_t)g.w.size());
+  }
+  const int64_t nrows = (int64_t)g.dst.size();
+  std::vector<int64_t> grow(nirr + 1, nrows);
+  for (int64_t row = nrows - 1; row >= 0; row--) grow[g.dst[row] / ncell] = row; // rows are grouped by block, in order
+  for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]); // blocks without rows
+  GhostDev &d = a->gt[which];
+  CUP2D_CUDA(upload(&d.rowptr, g.rowptr));
+  CUP2D_CUDA(upload(&d.dst, g.dst));
+  CUP2D_CUDA(upload(&d.sb, g.sb));
+  CUP2D_CUDA(upload(&d.sc, g.sc));
+  CUP2D_CUDA(upload(&d.w, g.w));
+  CUP2D_CUDA(upload(&d.grow, grow)); // last: marks the table complete
+  return CUP2D_OK;
+}
+
+// The fast kernels' tables of the blocks [gbegin, gbegin + nb), every block named by its slot (a distributed context's own
+// blocks first, then its halo slots).  The face fluxes of a distributed context travel in a field (flux_buf), so only a
+// plain context gets a buffer for them.
+int amr_fast_build(cup2d_amr *a) {
+  using namespace cup2d;
+  const int64_t b0 = a->gbegin, nb = a->nb;
+  std::vector<int32_t> n8, n4(4 * nb), irr_of(nb, -1);
+  int rc = plan_neighbours(a, n8);
+  if (rc) return rc;
+  for (int64_t k = 0; k < nb; k++) { // order of the 8: (-1,-1),(0,-1),(1,-1),(-1,0),(1,0),(-1,1),(0,1),(1,1)
+    const int pick[4] = {3, 4, 1, 6};  // W, E, S, N
+    for (int j = 0; j < 4; j++) {
+      const int32_t g = n8[8 * (b0 + k) + pick[j]];
+      n4[4 * k + j] = g < -1 ? -2 : g < 0 ? g : a->slot(g);
+      if (g >= 0 && n4[4 * k + j] < 0) return CUP2D_EINVAL; // a block the halo set missed
+    }
+  }
+  int64_t nirr = 0;
+  for (int32_t g : plan_irregular(a))
+    if (g >= b0 && g < b0 + nb) irr_of[g - b0] = (int32_t)nirr++;
+  a->nirr = nirr;
+  for (int which = 0; which < 3; which++)
+    if ((rc = amr_ghost_rows(a, which))) return rc;
+  CUP2D_CUDA(upload(&a->d_nbr4, n4));
+  CUP2D_CUDA(upload(&a->d_irr_of, irr_of));
+  if (!a->dist) CUP2D_CUDA(cudaMalloc(&a->d_faceflux, std::max<int64_t>(nirr, 1) * 64 * sizeof(double)));
+  return fast_constants();
+}
 
 int amr_advect_rhs_fast(cup2d_amr *a, double dt, const double *ddt) {
   using namespace cup2d;
@@ -422,123 +471,6 @@ int amr_pressure_gradient_fast(cup2d_amr *a, double dt, const double *ddt) {
   });
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;
-}
-
-// The compact ghost rows of one stencil kind for a DISTRIBUTED context: the plan's rows of the irregular blocks in this
-// rank's range, renumbered to the rank's irregular list (local position * ncell + lab entry), sources to local slots.
-int amr_ghosts_dist(cup2d_amr *a, int which, int ncell, cup2d::GhostDev &g) {
-  using namespace cup2d;
-  const int64_t b0 = a->gbegin, b1 = a->gbegin + a->nb;
-  const int64_t nirr_g = cup2d_amr_plan_irregular(a->plan, nullptr);
-  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1)), local_of_irr(std::max<int64_t>(nirr_g, 1), -1);
-  cup2d_amr_plan_irregular(a->plan, irr.data());
-  int64_t nirr = 0;
-  for (int64_t qi = 0; qi < nirr_g; qi++)
-    if (irr[qi] >= b0 && irr[qi] < b1) local_of_irr[qi] = (int32_t)nirr++;
-  int64_t nrows_g = 0;
-  const int64_t nnz_g = cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, nullptr, nullptr, nullptr, nullptr, nullptr);
-  if (nnz_g < 0) return CUP2D_EINVAL;
-  std::vector<int64_t> rp_g(nrows_g + 1);
-  std::vector<int32_t> dst_g(std::max<int64_t>(nrows_g, 1)), sb_g(std::max<int64_t>(nnz_g, 1)), sc_g(std::max<int64_t>(nnz_g, 1));
-  std::vector<double> w_g(std::max<int64_t>(nnz_g, 1));
-  cup2d_amr_plan_ghosts(a->plan, which, &nrows_g, rp_g.data(), dst_g.data(), sb_g.data(), sc_g.data(), w_g.data());
-  std::vector<int64_t> rp(1, 0);
-  std::vector<int32_t> dst, sb, sc;
-  std::vector<double> w;
-  for (int64_t row = 0; row < nrows_g; row++) {
-    const int32_t ql = local_of_irr[dst_g[row] / ncell];
-    if (ql < 0) continue;
-    dst.push_back(ql * ncell + dst_g[row] % ncell);
-    for (int64_t e = rp_g[row]; e < rp_g[row + 1]; e++) {
-      const int32_t sl = a->slot_of[sb_g[e]];
-      if (sl < 0) {
-        set_error("distributed context: a lab source lies outside the halo set");
-        return CUP2D_EINVAL;
-      }
-      sb.push_back(sl);
-      sc.push_back(sc_g[e]);
-      w.push_back(w_g[e]);
-    }
-    rp.push_back((int64_t)w.size());
-  }
-  const int64_t nrows = (int64_t)dst.size();
-  std::vector<int64_t> grow(nirr + 1, nrows);
-  for (int64_t row = nrows - 1; row >= 0; row--) grow[dst[row] / ncell] = row;
-  for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]);
-  auto up = [](auto **d, const auto &h) -> cudaError_t {
-    using T = typename std::remove_reference<decltype(h[0])>::type;
-    cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  };
-  CUP2D_CUDA(up(&g.rowptr, rp));
-  CUP2D_CUDA(up(&g.dst, dst));
-  CUP2D_CUDA(up(&g.sb, sb));
-  CUP2D_CUDA(up(&g.sc, sc));
-  CUP2D_CUDA(up(&g.w, w));
-  CUP2D_CUDA(up(&g.grow, grow)); // last: marks the table complete
-  return CUP2D_OK;
-}
-
-// Tables of a DISTRIBUTED context: the plan knows the whole mesh; this rank keeps what concerns its blocks [b0, b1) and
-// names every block by its local slot (own blocks first, then the halo slots of the field arrays): slot_of[global block] or -1.
-int amr_fast_setup_dist(cup2d_amr *a, const std::vector<int32_t> &slot_of, int64_t b0, int64_t b1) {
-  using namespace cup2d;
-  const int64_t nglob = (int64_t)slot_of.size(), nloc = b1 - b0;
-  auto up = [](auto **d, const auto &h) -> cudaError_t {
-    using T = typename std::remove_reference<decltype(h[0])>::type;
-    cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  };
-  auto slot = [&](int32_t g) -> int32_t {
-    if (g < 0) return g;
-    return slot_of[g]; // -1 would mean a block the halo set missed: caught below
-  };
-  std::vector<int32_t> n8(8 * nglob), n4(4 * nloc);
-  if (cup2d_amr_plan_neighbours(a->plan, n8.data())) return CUP2D_EINVAL;
-  for (int64_t k = 0; k < nloc; k++) {
-    const int pick[4] = {3, 4, 1, 6}; // W, E, S, N
-    for (int j = 0; j < 4; j++) {
-      const int32_t g = n8[8 * (b0 + k) + pick[j]];
-      n4[4 * k + j] = g < -1 ? -2 : slot(g);
-      if (g >= 0 && n4[4 * k + j] < 0) return CUP2D_EINVAL;
-    }
-  }
-  const int64_t nirr_g = cup2d_amr_plan_irregular(a->plan, nullptr);
-  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1)), irr_of(nloc, -1);
-  cup2d_amr_plan_irregular(a->plan, irr.data());
-  int64_t nirr = 0;
-  for (int64_t qi = 0; qi < nirr_g; qi++)
-    if (irr[qi] >= b0 && irr[qi] < b1) irr_of[irr[qi] - b0] = (int32_t)nirr++;
-  a->nirr = nirr;
-  const int ncell[3] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10};
-  for (int which = 0; which < 3; which++) {
-    const int rc = amr_ghosts_dist(a, which, ncell[which], a->gt[which]);
-    if (rc) return rc;
-  }
-  CUP2D_CUDA(up(&a->d_nbr4, n4));
-  CUP2D_CUDA(up(&a->d_irr_of, irr_of));
-  // coarse faces whose COARSE block is ours (the fine side may be a halo slot)
-  const int64_t nf = cup2d_amr_plan_faces(a->plan, nullptr);
-  std::vector<int32_t> rec(5 * std::max<int64_t>(nf, 1));
-  cup2d_amr_plan_faces(a->plan, rec.data());
-  std::map<std::pair<int, int>, CoarseFace> byface;
-  for (int64_t r = 0; r < nf; r++) {
-    const int fine = rec[5 * r], kc = rec[5 * r + 2], fc = rec[5 * r + 3], half = rec[5 * r + 4];
-    if (kc < b0 || kc >= b1) continue;
-    auto it = byface.find({kc, fc});
-    if (it == byface.end()) it = byface.emplace(std::make_pair(kc, fc), CoarseFace{(int)(kc - b0), fc, {-1, -1}}).first;
-    it->second.fine[half] = slot(fine);
-    if (it->second.fine[half] < 0) return CUP2D_EINVAL;
-  }
-  std::vector<CoarseFace> lists[2];
-  for (auto &e : byface) lists[e.second.face < 2 ? 0 : 1].push_back(e.second);
-  for (int d = 0; d < 2; d++) {
-    a->ncf[d] = (int)lists[d].size();
-    if (!lists[d].empty()) CUP2D_CUDA(up(&a->d_cf[d], lists[d]));
-  }
-  return fast_constants();
 }
 
 using namespace cup2d;

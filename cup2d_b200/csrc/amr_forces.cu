@@ -33,15 +33,7 @@
 #include <cmath>
 #include <cstring>
 #include <string>
-#include <type_traits>
 #include <vector>
-
-extern "C" {
-int64_t cup2d_amr_plan_ghosts(cup2d_amr_plan *p, int which, int64_t *nrows, int64_t *rowptr, int32_t *dst, int32_t *src_block,
-                              int32_t *src_cellcomp, double *weight);
-int cup2d_amr_plan_neighbours(cup2d_amr_plan *p, int32_t *out);
-int64_t cup2d_amr_plan_irregular(cup2d_amr_plan *p, int32_t *blocks_out);
-}
 
 namespace cup2d {
 
@@ -330,53 +322,20 @@ static int fo_grow(void **p, size_t *cap, size_t bytes) {
 static int fo_tables(cup2d_amr *a) {
   int rc = amr_fast_tables(a);
   if (rc) return rc;
-  auto up = [](auto **d, const auto &h) -> cudaError_t {
-    using T = typename std::remove_reference<decltype(h[0])>::type;
-    cudaError_t e = cudaMalloc(d, std::max<size_t>(h.size(), 1) * sizeof(T));
-    if (e != cudaSuccess) return e;
-    return cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-  };
-  if (!a->d_nbr8) {
-    const int64_t nall = a->dist ? a->nglobal : a->nb;
-    std::vector<int32_t> n8((size_t)8 * nall);
-    if (cup2d_amr_plan_neighbours(a->plan, n8.data())) return CUP2D_EINVAL;
-    if (a->dist) { // this rank's rows, same-level neighbours by slot (the halo set holds them); walls and level jumps keep their codes
-      n8.erase(n8.begin(), n8.begin() + 8 * a->gbegin);
-      n8.resize((size_t)8 * a->nb);
-      for (auto &g : n8)
-        if (g >= 0 && (g = a->slot_of[g]) < 0) {
-          set_error("distributed context: a lab source lies outside the halo set");
-          return CUP2D_EINVAL;
-        }
-    }
-    CUP2D_CUDA(up(&a->d_nbr8, n8));
+  if (!a->d_nbr8) { // same-level neighbours by slot (the halo set holds them); walls and level jumps keep their codes
+    std::vector<int32_t> n8;
+    if ((rc = plan_neighbours(a, n8))) return rc;
+    n8.erase(n8.begin() + 8 * (a->gbegin + a->nb), n8.end());
+    n8.erase(n8.begin(), n8.begin() + 8 * a->gbegin);
+    for (auto &g : n8)
+      if (g >= 0 && (g = a->slot(g)) < 0) {
+        set_error("distributed context: a lab source lies outside the halo set");
+        return CUP2D_EINVAL;
+      }
+    CUP2D_CUDA(upload(&a->d_nbr8, n8));
   }
-  if (a->dist) {
-    for (int which : {3, 6})
-      if (!a->gt[which].grow && (rc = amr_ghosts_dist(a, which, which == 6 ? 16 * 16 * 2 : 16 * 16, a->gt[which]))) return rc;
-    return CUP2D_OK;
-  }
-  const int64_t nirr = cup2d_amr_plan_irregular(a->plan, nullptr);
-  for (int which : {3, 6}) {
-    GhostDev &g = a->gt[which];
-    if (g.grow) continue;
-    const int ncell = which == 6 ? 16 * 16 * 2 : 16 * 16;
-    int64_t nrows = 0;
-    const int64_t nnz = cup2d_amr_plan_ghosts(a->plan, which, &nrows, nullptr, nullptr, nullptr, nullptr, nullptr);
-    if (nnz < 0) return CUP2D_EINVAL;
-    std::vector<int64_t> rp(nrows + 1), grow(nirr + 1, nrows);
-    std::vector<int32_t> dst(std::max<int64_t>(nrows, 1)), sb(std::max<int64_t>(nnz, 1)), sc(std::max<int64_t>(nnz, 1));
-    std::vector<double> w(std::max<int64_t>(nnz, 1));
-    cup2d_amr_plan_ghosts(a->plan, which, &nrows, rp.data(), dst.data(), sb.data(), sc.data(), w.data());
-    for (int64_t row = nrows - 1; row >= 0; row--) grow[dst[row] / ncell] = row; // rows are grouped by block, in order
-    for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]);
-    CUP2D_CUDA(up(&g.rowptr, rp));
-    CUP2D_CUDA(up(&g.dst, dst));
-    CUP2D_CUDA(up(&g.sb, sb));
-    CUP2D_CUDA(up(&g.sc, sc));
-    CUP2D_CUDA(up(&g.w, w));
-    CUP2D_CUDA(up(&g.grow, grow)); // last: marks the table complete
-  }
+  for (int which : {3, 6})
+    if (!a->gt[which].grow && (rc = amr_ghost_rows(a, which))) return rc;
   return CUP2D_OK;
 }
 

@@ -268,45 +268,39 @@ __global__ void amr_fluxcorr_kernel(const CoarseFace *__restrict__ cf, int ncf, 
 static int grid_for(int64_t n) { return (int)std::min<int64_t>((n + 255) / 256, AMR_GRID_SMS * 16); }
 
 static int upload_csr(cup2d_amr *a, int which) {
-  int64_t nnz = cup2d_amr_plan_stencil(a->plan, which, nullptr, nullptr, nullptr, nullptr);
+  const int64_t nnz = cup2d_amr_plan_stencil(a->plan, which, nullptr, nullptr, nullptr, nullptr);
   if (nnz < 0) return CUP2D_EINVAL;
   const int64_t per_block = LABN[which] * LABN[which] * LABD[which];
   const int64_t nrows = a->nb * per_block;
-  std::vector<int64_t> rp((a->dist ? a->nglobal : a->nb) * per_block + 1);
+  std::vector<int64_t> rp(a->nglobal * per_block + 1);
   std::vector<int32_t> sb(nnz), sc(nnz);
   std::vector<double> w(nnz);
   cup2d_amr_plan_stencil(a->plan, which, rp.data(), sb.data(), sc.data(), w.data());
-  if (a->dist) { // the rows of this rank's blocks (contiguous: rows are in block order), sources renumbered to local slots
-    const int64_t r0 = a->gbegin * per_block, e0 = rp[r0], e1 = rp[r0 + nrows];
-    for (int64_t e = e0; e < e1; e++) {
-      sb[e] = a->slot_of[sb[e]];
-      if (sb[e] < 0) {
-        set_error("distributed context: a lab source lies outside the halo set");
-        return CUP2D_EINVAL;
-      }
+  // the rows of the context's blocks (contiguous: rows are in block order), sources renumbered to slots
+  const int64_t r0 = a->gbegin * per_block, e0 = rp[r0], e1 = rp[r0 + nrows];
+  for (int64_t e = e0; e < e1; e++) {
+    sb[e] = a->slot(sb[e]);
+    if (sb[e] < 0) {
+      set_error("distributed context: a lab source lies outside the halo set");
+      return CUP2D_EINVAL;
     }
-    std::vector<int64_t> rpl(nrows + 1);
-    for (int64_t r = 0; r <= nrows; r++) rpl[r] = rp[r0 + r] - e0;
-    rp.swap(rpl);
-    auto keep = [&](auto &v) {
-      v.erase(v.begin() + e1, v.end());
-      v.erase(v.begin(), v.begin() + e0);
-    };
-    keep(sb);
-    keep(sc);
-    keep(w);
-    nnz = e1 - e0;
   }
+  rp.erase(rp.begin() + r0 + nrows + 1, rp.end());
+  rp.erase(rp.begin(), rp.begin() + r0);
+  for (auto &r : rp) r -= e0;
+  auto keep = [&](auto &v) {
+    v.erase(v.begin() + e1, v.end());
+    v.erase(v.begin(), v.begin() + e0);
+  };
+  keep(sb);
+  keep(sc);
+  keep(w);
   Csr &c = a->csr[which];
   c.nrows = nrows;
-  CUP2D_CUDA(cudaMalloc(&c.rowptr, (nrows + 1) * sizeof(int64_t)));
-  CUP2D_CUDA(cudaMalloc(&c.src_block, std::max<int64_t>(nnz, 1) * sizeof(int)));
-  CUP2D_CUDA(cudaMalloc(&c.src_cc, std::max<int64_t>(nnz, 1) * sizeof(int)));
-  CUP2D_CUDA(cudaMalloc(&c.w, std::max<int64_t>(nnz, 1) * sizeof(double)));
-  CUP2D_CUDA(cudaMemcpy(c.rowptr, rp.data(), (nrows + 1) * sizeof(int64_t), cudaMemcpyHostToDevice));
-  CUP2D_CUDA(cudaMemcpy(c.src_block, sb.data(), nnz * sizeof(int), cudaMemcpyHostToDevice));
-  CUP2D_CUDA(cudaMemcpy(c.src_cc, sc.data(), nnz * sizeof(int), cudaMemcpyHostToDevice));
-  CUP2D_CUDA(cudaMemcpy(c.w, w.data(), nnz * sizeof(double), cudaMemcpyHostToDevice));
+  CUP2D_CUDA(upload(&c.rowptr, rp));
+  CUP2D_CUDA(upload(&c.src_block, sb));
+  CUP2D_CUDA(upload(&c.src_cc, sc));
+  CUP2D_CUDA(upload(&c.w, w));
   CUP2D_CUDA(cudaMalloc(&a->lab[which], nrows * sizeof(double)));
   return CUP2D_OK;
 }
@@ -340,6 +334,46 @@ static int fluxcorr(cup2d_amr *a, const double *labA, const double *labB, double
     });
   }
   CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
+}
+
+// The cell size of every block the context holds (own blocks and halo slots, nslots in all), the smallest cell of the whole
+// mesh (the time step's), the (i, j) of the own blocks, the per-block partials
+static int block_sizes(cup2d_amr *a, const int32_t *level_ij, int64_t nslots) {
+  std::vector<double> h(nslots, a->h0);
+  a->hmin = a->h0;
+  for (int64_t g = 0; g < a->nglobal; g++) {
+    const double hg = a->h0 / (double)(1 << level_ij[3 * g]);
+    a->hmin = std::min(a->hmin, hg);
+    if (a->slot(g) >= 0) h[a->slot(g)] = hg;
+  }
+  const int32_t *own = level_ij + 3 * a->gbegin;
+  a->h_ij.resize(2 * a->nb);
+  for (int64_t k = 0; k < a->nb; k++) a->h_ij[2 * k] = own[3 * k + 1], a->h_ij[2 * k + 1] = own[3 * k + 2];
+  a->h_part.resize(2 * a->nb);
+  if (cudaMalloc(&a->d_part, 2 * a->nb * sizeof(double)) != cudaSuccess || upload(&a->d_h, h) != cudaSuccess) return CUP2D_ECUDA;
+  return CUP2D_OK;
+}
+
+// The coarse faces of the context's blocks: the plan's (fine block, face, coarse block, face, half) records grouped by
+// (coarse block, face), the fine side by slot (on a distributed context it may be a halo slot)
+static int coarse_faces(cup2d_amr *a) {
+  const std::vector<int32_t> rec = plan_faces(a);
+  const int64_t b0 = a->gbegin, b1 = a->gbegin + a->nb;
+  std::map<std::pair<int, int>, CoarseFace> byface;
+  for (size_t r = 0; r < rec.size(); r += 5) {
+    const int fine = rec[r], kc = rec[r + 2], fc = rec[r + 3], half = rec[r + 4];
+    if (kc < b0 || kc >= b1) continue;
+    auto it = byface.find({kc, fc});
+    if (it == byface.end()) it = byface.emplace(std::make_pair(kc, fc), CoarseFace{(int)(kc - b0), fc, {-1, -1}}).first;
+    if ((it->second.fine[half] = a->slot(fine)) < 0) return CUP2D_EINVAL;
+  }
+  std::vector<CoarseFace> lists[2];
+  for (auto &e : byface) lists[e.second.face < 2 ? 0 : 1].push_back(e.second);
+  for (int d = 0; d < 2; d++) {
+    a->ncf[d] = (int)lists[d].size();
+    if (!lists[d].empty()) CUP2D_CUDA(upload(&a->d_cf[d], lists[d]));
+  }
   return CUP2D_OK;
 }
 
@@ -386,7 +420,7 @@ int cup2d_amr_create(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int
   if (rc) return rc;
   cup2d_amr *a = new cup2d_amr;
   a->plan = plan;
-  a->nb = nblocks;
+  a->nb = a->nglobal = nblocks;
   a->device = device;
   a->h0 = h0;
   a->nu = nu;
@@ -405,36 +439,8 @@ int cup2d_amr_create(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int
       return fail(CUP2D_ECUDA);
     }
   }
-  std::vector<double> h(nblocks);
-  for (int64_t k = 0; k < nblocks; k++) h[k] = h0 / (double)(1 << level_ij[3 * k]);
-  a->h_ij.resize(2 * nblocks);
-  for (int64_t k = 0; k < nblocks; k++) a->h_ij[2 * k] = level_ij[3 * k + 1], a->h_ij[2 * k + 1] = level_ij[3 * k + 2];
-  a->hmin = *std::min_element(h.begin(), h.end());
-  a->h_part.resize(2 * nblocks);
-  if (cudaMalloc(&a->d_part, 2 * nblocks * sizeof(double)) != cudaSuccess) return fail(CUP2D_ECUDA);
-  if (cudaMalloc(&a->d_h, nblocks * sizeof(double)) != cudaSuccess ||
-      cudaMemcpy(a->d_h, h.data(), nblocks * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
-    return fail(CUP2D_ECUDA);
-  // coarse faces: group the plan's (fine block, face, coarse block, face, half) records by (coarse block, face)
-  const int64_t nf = cup2d_amr_plan_faces(plan, nullptr);
-  std::vector<int32_t> rec(5 * std::max<int64_t>(nf, 1));
-  cup2d_amr_plan_faces(plan, rec.data());
-  std::map<std::pair<int, int>, CoarseFace> byface;
-  for (int64_t r = 0; r < nf; r++) {
-    const int fine = rec[5 * r], kc = rec[5 * r + 2], fc = rec[5 * r + 3], half = rec[5 * r + 4];
-    auto it = byface.find({kc, fc});
-    if (it == byface.end()) it = byface.emplace(std::make_pair(kc, fc), CoarseFace{kc, fc, {-1, -1}}).first;
-    it->second.fine[half] = fine;
-  }
-  std::vector<CoarseFace> lists[2];
-  for (auto &e : byface) lists[e.second.face < 2 ? 0 : 1].push_back(e.second);
-  for (int d = 0; d < 2; d++) {
-    a->ncf[d] = (int)lists[d].size();
-    if (lists[d].empty()) continue;
-    if (cudaMalloc(&a->d_cf[d], lists[d].size() * sizeof(CoarseFace)) != cudaSuccess ||
-        cudaMemcpy(a->d_cf[d], lists[d].data(), lists[d].size() * sizeof(CoarseFace), cudaMemcpyHostToDevice) != cudaSuccess)
-      return fail(CUP2D_ECUDA);
-  }
+  // the baseline kernels' flux correction reads the coarse faces too: they are built here, not with the fast tables
+  if ((rc = block_sizes(a, level_ij, nblocks)) || (rc = coarse_faces(a))) return fail(rc);
   *out = a;
   return CUP2D_OK;
 }
@@ -792,6 +798,32 @@ static bool valid_partition(int64_t nblocks, int32_t nranks, const int64_t *rank
   return true;
 }
 
+// The Poisson rows (cup2d_amr_plan_poisson) of the blocks [b0, b1) of the plan's list, as cup2d_poisson_create_general_ranks
+// takes them: the blocks' face neighbours, their general rows numbered from the range's first cell, columns global.
+// [0, nglobal) gives the plan's arrays unchanged.
+struct PoissonRows {
+  std::vector<int32_t> nbr, rows, rowptr, col;
+  std::vector<double> val;
+};
+static int poisson_rows(cup2d_amr *a, int64_t b0, int64_t b1, PoissonRows &q) {
+  int64_t nnz = 0;
+  const int64_t nr = cup2d_amr_plan_poisson(a->plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
+  if (nr < 0) return (int)nr;
+  q.nbr.resize(4 * a->nglobal), q.rows.resize(nr), q.rowptr.resize(nr + 1), q.col.resize(nnz), q.val.resize(nnz);
+  cup2d_amr_plan_poisson(a->plan, q.nbr.data(), &nnz, q.rows.data(), q.rowptr.data(), q.col.data(), q.val.data());
+  const int64_t k0 = std::lower_bound(q.rows.begin(), q.rows.end(), (int32_t)(64 * b0)) - q.rows.begin();
+  const int64_t k1 = std::lower_bound(q.rows.begin(), q.rows.end(), (int32_t)(64 * b1)) - q.rows.begin();
+  const int32_t e0 = q.rowptr[k0], e1 = q.rowptr[k1];
+  auto keep = [](auto &v, int64_t i0, int64_t i1) {
+    v.erase(v.begin() + i1, v.end());
+    v.erase(v.begin(), v.begin() + i0);
+  };
+  keep(q.nbr, 4 * b0, 4 * b1), keep(q.rows, k0, k1), keep(q.rowptr, k0, k1 + 1), keep(q.col, e0, e1), keep(q.val, e0, e1);
+  for (auto &r : q.rows) r -= (int32_t)(64 * b0);
+  for (auto &e : q.rowptr) e -= e0;
+  return CUP2D_OK;
+}
+
 int cup2d_amr_create_ranks(int64_t nblocks, const int32_t *level_ij, int32_t bpdx, int32_t bpdy, double h0, double nu, int32_t rank,
                            int32_t nranks, const int64_t *rank_begin, int32_t device, cup2d_amr **out) {
   if (!out || !level_ij || !(h0 > 0) || rank < 0 || rank >= nranks || !valid_partition(nblocks, nranks, rank_begin)) {
@@ -820,77 +852,37 @@ int cup2d_amr_create_ranks(int64_t nblocks, const int32_t *level_ij, int32_t bpd
   a->nglobal = nblocks;
   // every remote block the stencil tables of this rank name: face neighbours, sources of its ghost rows, fine sides of its
   // coarse faces (the Poisson rows add theirs inside the constructor below)
-  std::vector<int32_t> extra, n8(8 * nblocks);
-  if (cup2d_amr_plan_neighbours(plan, n8.data())) return fail(CUP2D_EINVAL);
+  std::vector<int32_t> extra, n8;
+  if ((rc = plan_neighbours(a, n8))) return fail(rc);
   for (int64_t k = b0; k < b1; k++)
     for (int j = 0; j < 8; j++)
       if (n8[8 * k + j] >= 0) extra.push_back(n8[8 * k + j]);
-  const int64_t nirr_g = cup2d_amr_plan_irregular(plan, nullptr);
-  std::vector<int32_t> irr(std::max<int64_t>(nirr_g, 1));
-  cup2d_amr_plan_irregular(plan, irr.data());
-  // kinds 0-3 and 6 (3: the chi lab of the tagging rule and of the forces, 6: the forces' velocity lab)
-  const int kinds[5] = {0, 1, 2, 3, 6}, ncells[5] = {14 * 14 * 2, 10 * 10 * 2, 10 * 10, 16 * 16, 16 * 16 * 2};
-  for (int kk = 0; kk < 5; kk++) {
-    const int which = kinds[kk], ncell = ncells[kk];
-    int64_t nrows = 0;
-    const int64_t nnz = cup2d_amr_plan_ghosts(plan, which, &nrows, nullptr, nullptr, nullptr, nullptr, nullptr);
-    if (nnz < 0) return fail(CUP2D_EINVAL);
-    std::vector<int64_t> rp(nrows + 1);
-    std::vector<int32_t> dst(std::max<int64_t>(nrows, 1)), sb(std::max<int64_t>(nnz, 1)), sc(std::max<int64_t>(nnz, 1));
-    std::vector<double> w(std::max<int64_t>(nnz, 1));
-    cup2d_amr_plan_ghosts(plan, which, &nrows, rp.data(), dst.data(), sb.data(), sc.data(), w.data());
-    for (int64_t row = 0; row < nrows; row++) {
-      const int32_t blk = irr[dst[row] / ncell];
+  const std::vector<int32_t> irr = plan_irregular(a);
+  for (int which : {0, 1, 2, 3, 6}) { // 3: the chi lab of the tagging rule and of the forces, 6: the forces' velocity lab
+    PlanGhosts g;
+    if ((rc = plan_ghosts(a, which, g))) return fail(rc);
+    for (size_t row = 0; row < g.dst.size(); row++) {
+      const int32_t blk = irr[g.dst[row] / GHOST_NCELL[which]];
       if (blk < b0 || blk >= b1) continue;
-      for (int64_t e = rp[row]; e < rp[row + 1]; e++) extra.push_back(sb[e]);
+      for (int64_t e = g.rowptr[row]; e < g.rowptr[row + 1]; e++) extra.push_back(g.sb[e]);
     }
   }
-  {
-    const int64_t nf = cup2d_amr_plan_faces(plan, nullptr);
-    std::vector<int32_t> rec(5 * std::max<int64_t>(nf, 1));
-    cup2d_amr_plan_faces(plan, rec.data());
-    for (int64_t r = 0; r < nf; r++)
-      if (rec[5 * r + 2] >= b0 && rec[5 * r + 2] < b1) extra.push_back(rec[5 * r]);
-  }
-  // this rank's rows of the Poisson matrix (as cup2d_amr_set_ranks)
-  int64_t nnz = 0;
-  const int64_t nr = cup2d_amr_plan_poisson(plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
-  if (nr < 0) return fail((int)nr);
-  std::vector<int32_t> nbr(4 * nblocks), rows(std::max<int64_t>(nr, 1)), rowptr(nr + 1), col(std::max<int64_t>(nnz, 1));
-  std::vector<double> val(std::max<int64_t>(nnz, 1));
-  cup2d_amr_plan_poisson(plan, nbr.data(), &nnz, rows.data(), rowptr.data(), col.data(), val.data());
-  const int64_t k0 = std::lower_bound(rows.begin(), rows.begin() + nr, (int32_t)(64 * b0)) - rows.begin();
-  const int64_t k1 = std::lower_bound(rows.begin(), rows.begin() + nr, (int32_t)(64 * b1)) - rows.begin();
-  std::vector<int32_t> my_rows(rows.begin() + k0, rows.begin() + k1), my_ptr(rowptr.begin() + k0, rowptr.begin() + k1 + 1);
-  for (auto &r : my_rows) r -= (int32_t)(64 * b0);
-  const int32_t e0 = my_ptr[0];
-  for (auto &e : my_ptr) e -= e0;
-  if ((rc = poisson_create_general_ranks_ex(nblocks, rank, nranks, rank_begin, nbr.data() + 4 * b0, k1 - k0, my_rows.data(),
-                                            my_ptr.data(), col.data() + e0, val.data() + e0, (int64_t)extra.size(), extra.data(),
+  const std::vector<int32_t> rec = plan_faces(a);
+  for (size_t r = 0; r < rec.size(); r += 5)
+    if (rec[r + 2] >= b0 && rec[r + 2] < b1) extra.push_back(rec[r]);
+  PoissonRows q; // this rank's rows of the Poisson matrix (as cup2d_amr_set_ranks)
+  if ((rc = poisson_rows(a, b0, b1, q))) return fail(rc);
+  if ((rc = poisson_create_general_ranks_ex(nblocks, rank, nranks, rank_begin, q.nbr.data(), (int64_t)q.rows.size(), q.rows.data(),
+                                            q.rowptr.data(), q.col.data(), q.val.data(), (int64_t)extra.size(), extra.data(),
                                             device, &a->poisson)))
     return fail(rc);
   cup2d_sim *ps = a->poisson;
   a->stream = ps->stream;
   for (int f = 0; f < CUP2D_NFIELDS; f++) a->f[f] = ps->f[f];
-  std::vector<int32_t> slot_of(nblocks, -1);
-  for (int64_t k = 0; k < nloc; k++) slot_of[b0 + k] = (int32_t)k;
-  for (int64_t k = 0; k < ps->nhalo; k++) slot_of[ps->halo_gid[k]] = (int32_t)(nloc + k);
-  a->slot_of = slot_of;
-  // cell size: own blocks and halo slots; the time step uses the smallest cell of the WHOLE mesh
-  std::vector<double> h(ps->nslots, h0);
-  a->hmin = h0;
-  for (int64_t g = 0; g < nblocks; g++) {
-    const double hg = h0 / (double)(1 << level_ij[3 * g]);
-    a->hmin = std::min(a->hmin, hg);
-    if (slot_of[g] >= 0) h[slot_of[g]] = hg;
-  }
-  a->h_ij.resize(2 * nloc);
-  for (int64_t k = 0; k < nloc; k++) a->h_ij[2 * k] = level_ij[3 * (b0 + k) + 1], a->h_ij[2 * k + 1] = level_ij[3 * (b0 + k) + 2];
-  a->h_part.resize(2 * nloc);
-  if (cudaMalloc(&a->d_part, 2 * nloc * sizeof(double)) != cudaSuccess || cudaMalloc(&a->d_h, h.size() * sizeof(double)) != cudaSuccess ||
-      cudaMemcpy(a->d_h, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess)
-    return fail(CUP2D_ECUDA);
-  if ((rc = amr_fast_setup_dist(a, slot_of, b0, b1))) return fail(rc);
+  a->slot_of.assign(nblocks, -1);
+  for (int64_t k = 0; k < nloc; k++) a->slot_of[b0 + k] = (int32_t)k;
+  for (int64_t k = 0; k < ps->nhalo; k++) a->slot_of[ps->halo_gid[k]] = (int32_t)(nloc + k);
+  if ((rc = block_sizes(a, level_ij, ps->nslots)) || (rc = coarse_faces(a)) || (rc = amr_fast_build(a))) return fail(rc);
   *out = a;
   return CUP2D_OK;
 }
@@ -906,22 +898,11 @@ int cup2d_amr_set_ranks(cup2d_amr *a, int32_t rank, int32_t nranks, const int64_
     return CUP2D_EINVAL;
   }
   CUP2D_CUDA(cudaSetDevice(a->device));
-  int64_t nnz = 0;
-  const int64_t nr = cup2d_amr_plan_poisson(a->plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
-  if (nr < 0) return (int)nr;
-  std::vector<int32_t> nbr(4 * a->nb), rows(std::max<int64_t>(nr, 1)), rowptr(nr + 1), col(std::max<int64_t>(nnz, 1));
-  std::vector<double> val(std::max<int64_t>(nnz, 1));
-  cup2d_amr_plan_poisson(a->plan, nbr.data(), &nnz, rows.data(), rowptr.data(), col.data(), val.data());
-  const int64_t b0 = rank_begin[rank], b1 = rank_begin[rank + 1];
-  const int64_t k0 = std::lower_bound(rows.begin(), rows.begin() + nr, (int32_t)(64 * b0)) - rows.begin();
-  const int64_t k1 = std::lower_bound(rows.begin(), rows.begin() + nr, (int32_t)(64 * b1)) - rows.begin();
-  std::vector<int32_t> my_rows(rows.begin() + k0, rows.begin() + k1), my_ptr(rowptr.begin() + k0, rowptr.begin() + k1 + 1);
-  for (auto &r : my_rows) r -= (int32_t)(64 * b0);
-  const int32_t e0 = my_ptr[0];
-  for (auto &e : my_ptr) e -= e0;
-  int rc = cup2d_poisson_create_general_ranks(a->nb, rank, nranks, rank_begin, nbr.data() + 4 * b0, k1 - k0, my_rows.data(),
-                                              my_ptr.data(), col.data() + e0, val.data() + e0, a->device, &a->poisson);
-  if (rc) return rc;
+  PoissonRows q;
+  int rc = poisson_rows(a, rank_begin[rank], rank_begin[rank + 1], q);
+  if (rc || (rc = cup2d_poisson_create_general_ranks(a->nb, rank, nranks, rank_begin, q.nbr.data(), (int64_t)q.rows.size(), q.rows.data(),
+                                                     q.rowptr.data(), q.col.data(), q.val.data(), a->device, &a->poisson)))
+    return rc;
   a->rank = rank;
   a->nranks = nranks;
   a->rank_begin.assign(rank_begin, rank_begin + nranks + 1);
@@ -977,14 +958,11 @@ static int poisson_solve_distributed(cup2d_amr *a, double tol_abs, double tol_re
 // the general-rows Poisson context over the blocks of the mesh, created on first use
 static int ensure_poisson(cup2d_amr *a) {
   if (a->poisson) return CUP2D_OK;
-  int64_t nnz = 0;
-  const int64_t nr = cup2d_amr_plan_poisson(a->plan, nullptr, &nnz, nullptr, nullptr, nullptr, nullptr);
-  if (nr < 0) return (int)nr;
-  std::vector<int32_t> nbr(4 * a->nb), rows(std::max<int64_t>(nr, 1)), rowptr(nr + 1), col(std::max<int64_t>(nnz, 1));
-  std::vector<double> val(std::max<int64_t>(nnz, 1));
-  cup2d_amr_plan_poisson(a->plan, nbr.data(), &nnz, rows.data(), rowptr.data(), col.data(), val.data());
-  return cup2d_poisson_create_general(a->nb, nbr.data(), nr, rows.data(), rowptr.data(), col.data(), val.data(), a->device,
-                                      &a->poisson);
+  PoissonRows q;
+  const int rc = poisson_rows(a, 0, a->nb, q);
+  if (rc) return rc;
+  return cup2d_poisson_create_general(a->nb, q.nbr.data(), (int64_t)q.rows.size(), q.rows.data(), q.rowptr.data(), q.col.data(),
+                                      q.val.data(), a->device, &a->poisson);
 }
 
 int cup2d_amr_poisson_solve(cup2d_amr *a, double tol_abs, double tol_rel, int max_restarts, int max_iter, int *iters,

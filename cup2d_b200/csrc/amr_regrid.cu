@@ -772,7 +772,7 @@ int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level
   }
   int bpdx = 0, bpdy = 0;
   const std::vector<int> &old = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
-  const int64_t nold = a->dist ? a->nglobal : a->nb; // a distributed context's plan holds the whole list
+  const int64_t nold = a->nglobal;
   if (a->dist) {
     std::vector<double> args = {1.0, (double)nblocks_new};
     list_hash(new_level_ij, nblocks_new, args);
@@ -867,7 +867,7 @@ int cup2d_amr_adapt(cup2d_amr *a, const double *block_linf, double rtol, double 
   }
   int bpdx = 0, bpdy = 0;
   const std::vector<int> &old = amr_plan_level_ij(a->plan, &bpdx, &bpdy);
-  const int64_t nold = a->dist ? a->nglobal : a->nb; // a distributed context's plan holds the whole list
+  const int64_t nold = a->nglobal;
   if (((int64_t)std::max(bpdx, bpdy) << (level_max - 1)) >= (1 << 29)) {
     set_error("cup2d_amr_adapt: the finest level has 2^29 blocks or more per direction");
     return CUP2D_EINVAL;

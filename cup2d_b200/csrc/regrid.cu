@@ -316,7 +316,7 @@ extern "C" int cup2d_amr_dump(cup2d_amr *a, double time, const char *path) {
   const int rc = amr_ensure_ij(a);
   if (rc) return rc;
   const bool dist = a->dist && a->nranks > 1; // every rank writes its own byte range, the last one the descriptor
-  return cup2d::dump_write(a->stream, a->f[CUP2D_VEL], a->d_ij, a->d_h, 0, a->nb, dist ? a->gbegin : 0,
-                           dist ? a->nglobal : a->nb, !dist || a->rank == a->nranks - 1, O_CREAT | O_WRONLY | (dist ? 0 : O_TRUNC),
+  return cup2d::dump_write(a->stream, a->f[CUP2D_VEL], a->d_ij, a->d_h, 0, a->nb, a->gbegin, a->nglobal,
+                           !dist || a->rank == a->nranks - 1, O_CREAT | O_WRONLY | (dist ? 0 : O_TRUNC),
                            cup2d::AMR_GRID_SMS * 8, "cup2d_amr_dump", time, path, nullptr);
 }
