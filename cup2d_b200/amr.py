@@ -281,7 +281,9 @@ class AmrSimulation:
         _l.check(self.lib.cup2d_amr_dump(self._h, float(time), os.fsencode(path)))
 
     def adapt_tags(self, rtol, level_max):
-        """per-block L-inf of adapt()'s tagging field (vorticity + the chi rule); the field itself is left in tmp"""
+        """per-block L-inf of adapt()'s tagging field (vorticity + the chi rule); the field itself is left in tmp.  Fast and
+        distributed contexts run one fused kernel on the compact ghost tables and build no per-cell table; baseline-mode
+        contexts gather through the full per-cell tables (built on first use); both give the same bits"""
         out = np.empty(len(self.blocks))
         _l.check(self.lib.cup2d_amr_adapt_tags(self._h, float(rtol), int(level_max), out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
@@ -301,7 +303,8 @@ class AmrSimulation:
         """adapt() on the device-resident fields in one call (cup2d_amr_adapt): tags (or the caller's per-block `block_linf`),
         decision, order and transfer on the device, the same mesh and fields as adapt_tags -> adapt_mesh -> regrid; returns
         whether the mesh changed (on a distributed context: the mesh or the partition, and `block_linf` holds this rank's
-        blocks; `dist` re-attaches the peers and `blocks` becomes this rank's new range)"""
+        blocks; `dist` re-attaches the peers and `blocks` becomes this rank's new range).  Without `block_linf` the tags are
+        adapt_tags', so on fast and distributed contexts no per-cell table is built"""
         linf = None
         if block_linf is not None:
             linf = np.ascontiguousarray(block_linf, dtype=np.float64)

@@ -117,8 +117,14 @@ extern "C" int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max);
 int amr_fast_tables(cup2d_amr *a);
 int amr_fast_build(cup2d_amr *a);
 // the compact ghost rows of stencil kind `which` of the context's irregular blocks into gt[which], every source by its slot
-// (csrc/amr_fast.cu); CUP2D_EINVAL if a source is not a halo slot
-int amr_ghost_rows(cup2d_amr *a, int which);
+// (csrc/amr_fast.cu); CUP2D_EINVAL if a source is not a halo slot.  source_order: into gt_src[which] instead, each row's
+// terms in the order of the full per-cell tables
+int amr_ghost_rows(cup2d_amr *a, int which, bool source_order = false);
+// the tables of the 16 x 16 chi / vel labs on first use (csrc/amr_fast.cu): the fast tables, d_nbr8 and gt[3]
+int amr_lab16_tables(cup2d_amr *a);
+// adapt()'s tagging on the fast kernels (csrc/amr_fast.cu): tmp and d_part as amr_adapt_tags_enqueue leaves them, from the
+// fast tables, d_nbr8 and the compact rows of kinds 1 and 3; h_finest is the cell size of level level_max - 1
+int amr_tags_fast(cup2d_amr *a, double rtol, double h_finest);
 // the per-block (i, j) table on the device, built on first use (csrc/penalize.cu)
 int amr_ensure_ij(cup2d_amr *a);
 // distributed contexts (cup2d_amr_create_ranks): refresh the halo slots of `field` from the owners (whole-block peer pulls,
@@ -139,7 +145,8 @@ struct cup2d_amr {
   cudaStream_t stream = nullptr;
   double *f[CUP2D_NFIELDS] = {};
   double *d_h = nullptr;            // cell size per block
-  cup2d::Csr csr[4];                // kinds 0-2 at creation, 3 (chi lab of the tagging rule) on first use
+  cup2d::Csr csr[4];                // full per-cell tables of the baseline kernels (kind 3: the tagging rule's chi lab), each
+                                    // on first use by a baseline-mode context; fast and distributed contexts never build them
   double *lab[4] = {};              // lab buffers per kind; a second kind-1 buffer for u_def
   double *lab_udef = nullptr;
   cup2d::CoarseFace *d_cf[2] = {};  // [0] x faces, [1] y faces
@@ -161,8 +168,9 @@ struct cup2d_amr {
   int *d_irr_of = nullptr;          // [nb] position in the irregular list or -1
   int64_t nirr = 0;
   cup2d::GhostDev gt[7];            // compact ghost tables per stencil kind (amr_ghost_rows): 0-2 with the fast tables,
-                                    // 3 and 6 (the force diagnostics' labs, csrc/amr_forces.cu) on first use
-  int *d_nbr8 = nullptr;            // [nb][8] cup2d_amr_plan_neighbours on the device (csrc/amr_forces.cu, first use)
+                                    // 3 (the 16 x 16 chi lab of tagging and forces) and 6 (the forces' vel lab) on first use
+  cup2d::GhostDev gt_src[4];        // kinds 1 and 3 with each row's terms in the full tables' order (the tagging kernel)
+  int *d_nbr8 = nullptr;            // [nb][8] cup2d_amr_plan_neighbours on the device (amr_lab16_tables, first use)
   double *d_faceflux = nullptr;     // [nirr][4 faces][8][2] face fluxes of the irregular blocks (single-rank contexts)
   // bodies (csrc/penalize.cu): per-shape obstacle blocks, a cup2d::Shape with
   // (d_dist, the signed distance, exists only for shapes placed by cup2d_amr_ongrid or given one by cup2d_amr_shape_set_dist;

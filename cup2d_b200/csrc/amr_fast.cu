@@ -263,6 +263,82 @@ amr_scalar_fast_kernel(const double *__restrict__ p, double *__restrict__ out, c
   }
 }
 
+// adapt()'s tagging (amr_vorticity_kernel + amr_tag_block_kernel of amr_ops.cu) without the full per-cell tables.  Does
+// block k's {-4,-4,5,5,tensorial} chi lab hold a positive value within `off` cells of the block?  Lanes stride over the lab
+// cells: own cells directly; on a regular block the ghosts from the 8-neighbour table with the scalar wall clamp (as fo_labs
+// in amr_forces.cu); on an irregular block the compact kind-3 rows, each summed in row order as amr_gather_kernel sums it.
+// Ghost cells the plan leaves unwritten are 0 in the full table and never fire.  Every lane gets the answer.
+__device__ __forceinline__ bool chi_fires(const double *__restrict__ chi, int k, int qi, int off, const int *__restrict__ nbr8,
+                                          const GhostDev &gc, int lane) {
+  auto inside = [off](int gx, int gy) { return gx >= -off && gx < 8 + off && gy >= -off && gy < 8 + off; };
+  const int *n8 = nbr8 + (size_t)k * 8; // (-1,-1),(0,-1),(1,-1),(-1,0),(1,0),(-1,1),(0,1),(1,1)
+  int hit = 0;
+  for (int c = lane; c < 256; c += 32) {
+    const int gx = (c & 15) - 4, gy = (c >> 4) - 4;
+    if (!inside(gx, gy)) continue;
+    const int ox = gx < 0 ? -1 : gx > 7, oy = gy < 0 ? -1 : gy > 7;
+    if (ox == 0 && oy == 0) {
+      hit |= chi[(size_t)k * 64 + gy * 8 + gx] > 0.0;
+      continue;
+    }
+    if (qi >= 0) continue; // irregular: the ghost rows below
+    const bool wx = ox != 0 && n8[ox < 0 ? 3 : 4] == -1, wy = oy != 0 && n8[oy < 0 ? 1 : 6] == -1;
+    const int cx = wx ? (ox < 0 ? 0 : 7) : gx, cy = wy ? (oy < 0 ? 0 : 7) : gy;
+    const int qx = cx < 0 ? -1 : cx > 7, qy = cy < 0 ? -1 : cy > 7;
+    const int b = qx == 0 && qy == 0 ? k : n8[(qy + 1) * 3 + (qx + 1) - ((qy + 1) * 3 + (qx + 1) > 4)];
+    hit |= chi[(size_t)b * 64 + (cy & 7) * 8 + (cx & 7)] > 0.0;
+  }
+  if (qi >= 0)
+    for (int64_t row = gc.grow[qi] + lane; row < gc.grow[qi + 1]; row += 32) {
+      const int c = gc.dst[row] % 256;
+      if (!inside((c & 15) - 4, (c >> 4) - 4)) continue;
+      double acc = 0.0;
+      for (int64_t e = gc.rowptr[row]; e < gc.rowptr[row + 1]; e++) acc += gc.w[e] * chi[(size_t)gc.sb[e] * 64 + gc.sc[e]];
+      hit |= acc > 0.0;
+    }
+  for (int m = 16; m; m >>= 1) hit |= __shfl_xor_sync(0xffffffffu, hit, m);
+  return hit != 0;
+}
+
+// tmp = KernelVorticity(vel) (main.cpp:3343-3366) with GradChiOnTmp's 2 Rtol in the four centre cells of the blocks whose chi
+// lab is positive within 4 cells (blocks of the finest level) or 2 (the others) (4631-4656); linf[k] = max |tmp| over block k
+// (4693-4697).  One warp owns four blocks: the +-1 lab of vel from load_lab1 (compact kind-1 rows), the chi test, then lane
+// (q, r) computes row r of block q in amr_vorticity_kernel's expression order.  Given ghost rows in the full tables' term
+// order, bit for bit the result of the table path.
+__global__ void __launch_bounds__(A1_NT)
+amr_tags_fast_kernel(const double *__restrict__ vel, const double *__restrict__ chi, double *__restrict__ tmp,
+                     const int4 *__restrict__ nbr4, const int *__restrict__ nbr8, const int *__restrict__ irr_of,
+                     const GhostDev gv, const GhostDev gc, const double *__restrict__ hb, double h_finest, double rtol,
+                     double *__restrict__ linf, int nb) {
+  __shared__ double s_lab[A1_WARPS * 4 * 2 * A1_PLANE];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, q = lane >> 3, r = lane & 7;
+  const int b0 = (blockIdx.x * A1_WARPS + warp) * 4;
+  if (b0 >= nb) return;
+  double *base = s_lab + warp * 4 * 2 * A1_PLANE;
+  bool fire = false; // block b0 + q
+  for (int qq = 0; qq < 4 && b0 + qq < nb; qq++) {
+    const int k = b0 + qq, qi = irr_of[k];
+    load_lab1<2>(base + qq * 2 * A1_PLANE, vel, k, nbr4[k], qi, gv, lane);
+    const bool f = chi_fires(chi, k, qi, hb[k] == h_finest ? 4 : 2, nbr8, gc, lane);
+    if (qq == q) fire = f;
+  }
+  const int k = b0 + q;
+  const bool live = k < nb;
+  const double *u = base + q * 2 * A1_PLANE, *v = u + A1_PLANE;
+  const double i2h = 0.5 / (live ? hb[k] : 1.0);
+  const int row = (r + 1) * A1_PS + 1;
+  double m = 0.0;
+  for (int i = 0; i < 8; i++) {
+    const int p = row + i;
+    double t = i2h * (((u[p - A1_PS] - u[p + A1_PS]) + v[p + 1]) - v[p - 1]);
+    if (fire && (r == 3 || r == 4) && (i == 3 || i == 4)) t = 2 * rtol;
+    if (live) tmp[(size_t)k * 64 + r * 8 + i] = t;
+    m = fmax(m, fabs(t));
+  }
+  for (int s = 4; s; s >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, s)); // the 8 rows of block q
+  if (live && r == 0) linf[k] = m;
+}
+
 // fillcases per coarse face from the stored face fluxes (see amr_fluxcorr_kernel in amr_ops.cu for the formulation)
 template <int DIM>
 __global__ void amr_fluxcorr_faces_kernel(const CoarseFace *__restrict__ cf, int ncf, const FluxBuf faceflux,
@@ -346,8 +422,10 @@ static int fast_setup(cup2d_amr *a) { return a->d_faceflux || a->dist ? CUP2D_OK
 int amr_fast_tables(cup2d_amr *a) { return cup2d::fast_setup(a); }
 
 // The plan's rows of the irregular blocks in [gbegin, gbegin + nb), renumbered to the context's irregular list (local
-// position * ncell + lab entry), every source by its slot.
-int amr_ghost_rows(cup2d_amr *a, int which) {
+// position * ncell + lab entry), every source by its slot.  source_order: each row's terms in ascending (block, cell) of the
+// whole list, the order of the full per-cell tables (cup2d_amr_plan_stencil), into gt_src[which]; the plan's compact rows
+// hold the same terms in the order of the block their pattern was made from.
+int amr_ghost_rows(cup2d_amr *a, int which, bool source_order) {
   using namespace cup2d;
   const int64_t b0 = a->gbegin, b1 = a->gbegin + a->nb;
   const int ncell = GHOST_NCELL[which];
@@ -362,11 +440,18 @@ int amr_ghost_rows(cup2d_amr *a, int which) {
   g.rowptr.reserve(all.rowptr.size()), g.dst.reserve(all.dst.size());
   g.sb.reserve(all.sb.size()), g.sc.reserve(all.sc.size()), g.w.reserve(all.w.size());
   g.rowptr.push_back(0);
+  std::vector<int64_t> terms;
   for (size_t row = 0; row < all.dst.size(); row++) {
     const int32_t ql = local_of_irr[all.dst[row] / ncell];
     if (ql < 0) continue;
     g.dst.push_back(ql * ncell + all.dst[row] % ncell);
-    for (int64_t e = all.rowptr[row]; e < all.rowptr[row + 1]; e++) {
+    terms.clear();
+    for (int64_t e = all.rowptr[row]; e < all.rowptr[row + 1]; e++) terms.push_back(e);
+    if (source_order)
+      std::sort(terms.begin(), terms.end(), [&](int64_t x, int64_t y) {
+        return all.sb[x] != all.sb[y] ? all.sb[x] < all.sb[y] : all.sc[x] < all.sc[y];
+      });
+    for (int64_t e : terms) {
       const int32_t sl = a->slot(all.sb[e]);
       if (sl < 0) {
         set_error("distributed context: a lab source lies outside the halo set");
@@ -382,7 +467,7 @@ int amr_ghost_rows(cup2d_amr *a, int which) {
   std::vector<int64_t> grow(nirr + 1, nrows);
   for (int64_t row = nrows - 1; row >= 0; row--) grow[g.dst[row] / ncell] = row; // rows are grouped by block, in order
   for (int64_t qi = nirr - 1; qi >= 0; qi--) grow[qi] = std::min(grow[qi], grow[qi + 1]); // blocks without rows
-  GhostDev &d = a->gt[which];
+  GhostDev &d = source_order ? a->gt_src[which] : a->gt[which];
   CUP2D_CUDA(upload(&d.rowptr, g.rowptr));
   CUP2D_CUDA(upload(&d.dst, g.dst));
   CUP2D_CUDA(upload(&d.sb, g.sb));
@@ -469,6 +554,43 @@ int amr_pressure_gradient_fast(cup2d_amr *a, double dt, const double *ddt) {
                                                              a->d_irr_of, a->gt[2], a->d_h, flux_buf<1>(a), (int)a->nb, d);
     return 0;
   });
+  CUP2D_CUDA(cudaGetLastError());
+  return CUP2D_OK;
+}
+
+// The tables of the 16 x 16 {-4,-4,5,5,tensorial} labs (the tagging kernel above, the force diagnostics of amr_forces.cu), on
+// first use and until a regrid: the fast tables, the 8-neighbour table and the compact ghost rows of kind 3.  A distributed
+// context keeps the rows of its own blocks and names every neighbour and source by its local slot.
+int amr_lab16_tables(cup2d_amr *a) {
+  using namespace cup2d;
+  int rc = fast_setup(a);
+  if (rc) return rc;
+  if (!a->d_nbr8) { // same-level neighbours by slot (the halo set holds them); walls and level jumps keep their codes
+    std::vector<int32_t> n8;
+    if ((rc = plan_neighbours(a, n8))) return rc;
+    n8.erase(n8.begin() + 8 * (a->gbegin + a->nb), n8.end());
+    n8.erase(n8.begin(), n8.begin() + 8 * a->gbegin);
+    for (auto &g : n8)
+      if (g >= 0 && (g = a->slot(g)) < 0) {
+        set_error("distributed context: a lab source lies outside the halo set");
+        return CUP2D_EINVAL;
+      }
+    CUP2D_CUDA(upload(&a->d_nbr8, n8));
+  }
+  return a->gt[3].grow ? CUP2D_OK : amr_ghost_rows(a, 3);
+}
+
+// adapt()'s tagging on the fast tables: tmp, and the per-block L-inf in d_part (vel and chi refreshed by the caller).  Its
+// ghost rows of kinds 1 and 3 sum their terms in the full tables' order (gt_src), so that every lab value is the baseline's.
+int amr_tags_fast(cup2d_amr *a, double rtol, double h_finest) {
+  using namespace cup2d;
+  int rc = amr_lab16_tables(a);
+  if (rc) return rc;
+  for (int which : {1, 3})
+    if (!a->gt_src[which].grow && (rc = amr_ghost_rows(a, which, true))) return rc;
+  const int grid = (int)((a->nb + A1_WARPS * 4 - 1) / (A1_WARPS * 4));
+  amr_tags_fast_kernel<<<grid, A1_NT, 0, a->stream>>>(a->f[CUP2D_VEL], a->f[CUP2D_CHI], a->f[CUP2D_TMP], reinterpret_cast<const int4 *>(a->d_nbr4),
+                                                      a->d_nbr8, a->d_irr_of, a->gt_src[1], a->gt_src[3], a->d_h, h_finest, rtol, a->d_part, (int)a->nb);
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;
 }

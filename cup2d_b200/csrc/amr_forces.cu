@@ -317,26 +317,12 @@ static int fo_grow(void **p, size_t *cap, size_t bytes) {
   return CUP2D_OK;
 }
 
-// the force labs' tables, on first use and until a regrid: the 8-neighbour table and the compact ghost rows of kinds 6 and 3.
-// A distributed context keeps the rows of its own blocks and names every neighbour and source by its local slot.
+// the force labs' tables, on first use and until a regrid: those of the 16 x 16 labs (the 8-neighbour table, kind 3) and the
+// compact ghost rows of kind 6
 static int fo_tables(cup2d_amr *a) {
-  int rc = amr_fast_tables(a);
+  int rc = amr_lab16_tables(a);
   if (rc) return rc;
-  if (!a->d_nbr8) { // same-level neighbours by slot (the halo set holds them); walls and level jumps keep their codes
-    std::vector<int32_t> n8;
-    if ((rc = plan_neighbours(a, n8))) return rc;
-    n8.erase(n8.begin() + 8 * (a->gbegin + a->nb), n8.end());
-    n8.erase(n8.begin(), n8.begin() + 8 * a->gbegin);
-    for (auto &g : n8)
-      if (g >= 0 && (g = a->slot(g)) < 0) {
-        set_error("distributed context: a lab source lies outside the halo set");
-        return CUP2D_EINVAL;
-      }
-    CUP2D_CUDA(upload(&a->d_nbr8, n8));
-  }
-  for (int which : {3, 6})
-    if (!a->gt[which].grow && (rc = amr_ghost_rows(a, which))) return rc;
-  return CUP2D_OK;
+  return a->gt[6].grow ? CUP2D_OK : amr_ghost_rows(a, 6);
 }
 
 static int fo_check(cup2d_amr *a, int nshapes, const char *who) {

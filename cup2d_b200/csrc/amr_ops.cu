@@ -310,7 +310,7 @@ static int upload_csr(cup2d_amr *a, int which) {
 // for them — they grow with the mesh, the compact ones with its level interfaces.
 static int gather(cup2d_amr *a, int which, const double *field, double *&lab) {
   int rc;
-  if (a->dist && which != 1 && which != 3) { // (1 and 3: the labs of the tagging field, whose sources are in the halo set)
+  if (a->dist) {
     set_error("this operator runs on the table-gather baseline kernels, which a distributed context does not have");
     return CUP2D_ESTATE;
   }
@@ -457,9 +457,11 @@ void cup2d_amr_destroy(cup2d_amr *a) {
   cudaFree(a->lab_udef); cudaFree(a->d_h); cudaFree(a->d_cf[0]); cudaFree(a->d_cf[1]); cudaFree(a->d_part);
   cudaFree(a->d_nbr4); cudaFree(a->d_nbr8); cudaFree(a->d_irr_of); cudaFree(a->d_faceflux); cudaFree(a->d_vsum);
   a->free_shapes();
-  for (auto &g : a->gt) {
+  auto free_ghosts = [](cup2d::GhostDev &g) {
     cudaFree(g.grow); cudaFree(g.rowptr); cudaFree(g.dst); cudaFree(g.sb); cudaFree(g.sc); cudaFree(g.w);
-  }
+  };
+  for (auto &g : a->gt) free_ghosts(g);
+  for (auto &g : a->gt_src) free_ghosts(g);
 #ifndef CUP2D_AMR_EMU
   amr_drop_graphs(a);
   if (a->ev_fork) cudaEventDestroy((cudaEvent_t)a->ev_fork);
@@ -567,16 +569,19 @@ static int block_partials(cup2d_amr *a, int n_per_block) {
 }
 
 /* adapt()'s per-block L-inf (main.cpp:4676-4697) on a multi-level mesh: vorticity of vel through the +-1 lab, the chi rule
- * of GradChiOnTmp through the {-4,-4,5,5,tensorial} chi lab (ghost tables built on first use); leaves the tagging field in
- * tmp like the reference does.  level_max = sim.levelMax (the finest level is level_max - 1). */
+ * of GradChiOnTmp through the {-4,-4,5,5,tensorial} chi lab; leaves the tagging field in tmp like the reference does.
+ * level_max = sim.levelMax (the finest level is level_max - 1).  Fast contexts (distributed ones included) run the fused
+ * kernel of amr_fast.cu on the compact tables; baseline-mode contexts gather both labs through the full per-cell tables
+ * (built on first use).  Both give the same bits. */
 int amr_adapt_tags_enqueue(cup2d_amr *a, double rtol, int level_max) {
   CUP2D_CUDA(cudaSetDevice(a->device));
   int rc;
   if ((rc = amr_dist_refresh(a, CUP2D_VEL)) || (rc = amr_dist_refresh(a, CUP2D_CHI))) return rc;
+  const double h_finest = a->h0 / (double)(1 << (level_max - 1));
+  if (a->fast) return amr_tags_fast(a, rtol, h_finest);
   if ((rc = gather(a, 1, a->f[CUP2D_VEL], a->lab[1])) || (rc = gather(a, 3, a->f[CUP2D_CHI], a->lab[3]))) return rc;
   amr_vorticity_kernel<<<grid_for(a->nb * 64), 256, 0, a->stream>>>(a->lab[1], a->f[CUP2D_TMP], a->d_h, a->nb * 64);
-  amr_tag_block_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->lab[3], a->f[CUP2D_TMP], a->d_h,
-                                                               a->h0 / (double)(1 << (level_max - 1)), rtol, a->d_part, a->nb);
+  amr_tag_block_kernel<<<grid_for(a->nb), 256, 0, a->stream>>>(a->lab[3], a->f[CUP2D_TMP], a->d_h, h_finest, rtol, a->d_part, a->nb);
   CUP2D_CUDA(cudaGetLastError());
   return CUP2D_OK;
 }

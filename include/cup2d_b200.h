@@ -358,7 +358,10 @@ int cup2d_amr_peer_attach(cup2d_amr *a, const void *all_blobs);
  * k of the field adapt() thresholds against Rtol / Ctol — the vorticity of vel (KernelVorticity, 3343-3366), with 2*rtol in
  * the four centre cells of every block whose chi lab (stencil {-4,-4,5,5,tensorial}, ghosts across level jumps included) is
  * positive within 4 cells (finest level, level_max - 1) or 2 cells (other levels) of it (GradChiOnTmp, 4631-4656).  The
- * field itself is left in tmp.  The decision is cup2d_amr_adapt_mesh, the field transfer cup2d_amr_regrid. */
+ * field itself is left in tmp.  The decision is cup2d_amr_adapt_mesh, the field transfer cup2d_amr_regrid.
+ * Fast contexts (cup2d_amr_set_fast) and distributed ones run one fused kernel on the compact ghost tables and build no
+ * per-cell table; baseline-mode contexts gather the labs through the full per-cell tables, built on first use.  Both give
+ * the same bits. */
 int cup2d_amr_adapt_tags(cup2d_amr *a, double rtol, int level_max, double *block_linf_out);
 
 /* dump() on a multi-level mesh (main.cpp:3367-3467; cf. cup2d_dump): path.xdmf2, path.xyz.raw, path.attr.raw — the
@@ -380,7 +383,8 @@ int64_t cup2d_amr_adapt_mesh(int64_t nblocks, const int32_t *level_ij, int32_t b
  * the ranks move onto the reference's new partition (see cup2d_amr_adapt) and read old blocks over the peer mapping. */
 int cup2d_amr_regrid(cup2d_amr *a, int64_t nblocks_new, const int32_t *new_level_ij);
 /* adapt() in one call, decision included (csrc/amr_regrid.cu): block_linf == NULL runs cup2d_amr_adapt_tags on the device
- * without downloading it (the tagging field is left in tmp as there); otherwise block_linf[nblocks] are the caller's per-block
+ * without downloading it (the tagging field is left in tmp as there; on fast and distributed contexts without any per-cell
+ * table); otherwise block_linf[nblocks] are the caller's per-block
  * values (host doubles; any criterion).  The refine / compress decision and the order of the new list are made on the device,
  * the same list as cup2d_amr_adapt_mesh; then the context is regridded in place as by cup2d_amr_regrid onto that list, with
  * the same fields.  Only the new block list and the refined parents cross to the host.  An unchanged list is a no-op after
